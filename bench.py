@@ -54,23 +54,23 @@ def peaks():
             return float(json.load(open(path))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (HBM3, 3.35 TB/s)'
 
 
-def ncu_traffic(workload, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` summary of the same workload (profiles/), or (None, None)."""
-    import glob
-    import re
-    for path in sorted(glob.glob(os.path.join(ROOT, 'profiles', f'r*_ncu_{kernel}_{workload}.txt')), reverse=True):
-        total, units = 0.0, {'Gbyte': 1e9, 'Mbyte': 1e6, 'Kbyte': 1e3, 'byte': 1.0, 'Tbyte': 1e12}
-        for line in open(path):
-            mt = re.match(r'\s*dram__bytes_(read|write)\.sum\s+([0-9.]+)\s+(\w+)', line)
-            if mt:
-                total += float(mt.group(2)) * units.get(mt.group(3), 1.0)
-        if total:
-            return total, os.path.relpath(path, ROOT)
-    return None, None
+DUMP_SAMPLE = 1 << 16   # elements sampled per output array by --dump-outputs
+
+
+def dump_outputs(out_dir, arrays, n):
+    """--dump-outputs: the last timed step's outputs as DIR/<name>.npy, sampled at one fixed, seeded set of element
+    indices; an element as its 32-bit words (least significant first) in float64, exact; a GF(2^8) element as its byte."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    idx = torch.from_numpy(np.sort(np.random.default_rng(20260923).choice(n, size=min(n, DUMP_SAMPLE), replace=False)))
+    for name, t in arrays.items():      # (..., n, L) int64 limbs, or (..., n) uint8
+        axis = t.dim() - (1 if t.dtype == torch.uint8 else 2)
+        a = t.index_select(axis, idx.to(t.device)).cpu().contiguous().numpy()
+        np.save(os.path.join(out_dir, name + '.npy'), (a if a.dtype == np.uint8 else a.view(np.uint32)).astype(np.float64))
 
 
 class ClockSampler:
@@ -166,13 +166,10 @@ def bind_to_gpu_numa(index):
 # ---------------------------------------------------------------------------------------------------
 
 def reference_path():
-    """Where the UNMODIFIED reference is importable from on this box: $MPYC_REFERENCE, or baseline/_ref (pip install
-    --target of the checkout, tools/install_reference.sh; git-ignored, travels with gpurun).  None: only the oracle
-    port (oracle/shamir_oracle.py) is available."""
-    for cand in (os.environ.get('MPYC_REFERENCE'), os.path.join(ROOT, 'baseline', '_ref')):
-        if cand and os.path.isfile(os.path.join(cand, 'mpyc', 'thresha.py')):
-            return cand
-    return None
+    """Where the UNMODIFIED reference is importable from: $MPYC_REFERENCE, or the copy build() makes in oracle/_ref
+    (oracle/reference.py).  None: only the oracle port (oracle/shamir_oracle.py) is available."""
+    from oracle import reference
+    return reference.path()
 
 
 _REFMOD = {}
@@ -232,7 +229,7 @@ def _cpu_pairs(args):
 
 
 def cpu_baseline(w, n=20000, target_s=12.0):
-    """1 core, bounded sample; returns the cpu_baseline object.  kind 'reference': mpyc.thresha itself (baseline/_ref
+    """1 core, bounded sample; returns the cpu_baseline object.  kind 'reference': mpyc.thresha itself (oracle/_ref
     or $MPYC_REFERENCE); kind 'port': oracle/shamir_oracle.py, its restatement pinned by the golden fixtures."""
     pairs, dt, kind = _cpu_pairs((w['p'], w['m'], w['t'], w['k'], n, 1, True))
     reps = max(1, int(target_s * 0.7 / max(dt, 1e-3)))
@@ -285,7 +282,7 @@ def workload_config(w, n, world):
 def run_reference_arm(a, w):
     """CPU arm: the reference's own thresha.np_random_split + np_recombine (NumPy object arrays, per-element
     secrets.randbelow) on all host cores, one independent process per core -- the UNMODIFIED reference when it is
-    importable on this box (baseline/_ref or $MPYC_REFERENCE: kind 'reference'), else the oracle port (kind 'port').
+    importable (oracle/_ref or $MPYC_REFERENCE: kind 'reference'), else the oracle port (kind 'port').
     Each step is a bounded sample of the workload: 20 000 pairs per process."""
     import multiprocessing as mp
     rank = int(os.environ.get('RANK', '0'))
@@ -370,7 +367,7 @@ def dropin_rate(w, device, n=200_000):
                           'wire_bytes_per_row': len(sent[0])}}
 
 
-def measure_prss(w, n, steps, warmup, local, rank, peak, with_e2e=True):
+def measure_prss(w, n, steps, warmup, local, rank, peak, with_e2e=True, dump_dir=None):
     """K4 on PRF bytes resident in HBM (CUDA events), and -- with_e2e -- the host pipeline mpyc_b200_prss_host and the
     drop-in call at np_cnnmnist's largest per-call size."""
     import itertools
@@ -415,6 +412,8 @@ def measure_prss(w, n, steps, warmup, local, rank, peak, with_e2e=True):
     torch.cuda.synchronize()
     t_end = time.perf_counter()
     launches = mpyc_b200.launch_count() - launches0
+    if dump_dir:
+        dump_outputs(dump_dir, {'shares': d_out}, n)
     ms = ev[0].elapsed_time(ev[-1]) / steps
     alg = n * (nsub * d * chunk + eb)
     ach = alg / (ms * 1e-3) / 1e9
@@ -465,7 +464,7 @@ def run_prss_arm(a, w):
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    r = measure_prss(w, n, a.steps, a.warmup, local, rank, peak)
+    r = measure_prss(w, n, a.steps, a.warmup, local, rank, peak, dump_dir=a.dump_outputs if rank == 0 else None)
     ms = r['ms']
     if world > 1:
         tt = torch.tensor([ms], device='cuda')
@@ -475,7 +474,7 @@ def run_prss_arm(a, w):
     sampler.stop()
     roofline = {'bound': 'hbm', 'kernel': 'k_prss_tiles', 'achieved': r['algorithmic_bytes'] / (ms * 1e-3) / 1e9, 'peak': peak,
                 'peak_source': peak_src, 'unit': 'GB/s', 'frac': r['algorithmic_bytes'] / (ms * 1e-3) / 1e9 / peak,
-                'traffic': ncu_traffic('prss', 'prss')[0], 'ms': ms, 'algorithmic_bytes': r['algorithmic_bytes'],
+                'ms': ms, 'algorithmic_bytes': r['algorithmic_bytes'],
                 'note': 'subset constants are cached in the field handle: a call costs no allocation, upload or synchronisation'}
     e2e = r['e2e']
     e2e['value'] *= world
@@ -498,7 +497,7 @@ def run_prss_arm(a, w):
                 'steps': a.steps, 'warmup': a.warmup, 'ms_per_step': ms, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
                 'dtype': f'u64x{r["ctx"].nlimbs} limbs (exact integer arithmetic mod p)', 'data': 'synthetic',
                 'config': {'workload': w['name'], 'p_bits': p.bit_length(), 'm': m, 't': t, 'subsets': r['nsub'], 'chunk_bytes': r['chunk'], 'n_per_gpu': n,
-                           'l2_policy': 'PRF bytes (2 GB) far larger than the 126 MB L2; no flush needed'},
+                           'l2_policy': 'PRF bytes (2 GB) far larger than the 50 MB L2; no flush needed'},
                 'roofline': roofline, 'cpu_baseline': cpu, 'e2e': e2e, 'gpu_launches': r['gpu_launches'], 'clocks': clocks}
         print(json.dumps(line), flush=True)
     if world > 1:
@@ -526,7 +525,7 @@ def _dist_init(local):
     return dist
 
 
-def measure_device(w, n, steps, warmup, seed_rank=0, sustain_s=0.0, keep=False):
+def measure_device(w, n, steps, warmup, seed_rank=0, sustain_s=0.0, keep=False, dump_dir=None):
     """K steps of the hot path on device-resident inputs, timed with CUDA events on the launching stream.
     Returns a dict with per-kernel milliseconds, launches and (keep=True) the buffers for later checks."""
     import torch
@@ -586,6 +585,8 @@ def measure_device(w, n, steps, warmup, seed_rank=0, sustain_s=0.0, keep=False):
     common = dict(ctx=ctx, is_mul=is_mul, eb=ctx.elem_bytes, L=max(ctx.nlimbs, 1))
     res = timed(steps)
     res.update(common)
+    if dump_dir:
+        dump_outputs(dump_dir, {'product': OUT.t} if is_mul else {'shares': SH.t, 'recombined': REC.t[0]}, n)
     if sustain_s > 0:
         per = max(res['total_ms'] / steps, 1e-3)
         res['sustained'] = timed(max(steps, int(sustain_s * 1e3 / per) + 1))
@@ -838,7 +839,8 @@ def run_gpu_arm(a, w):
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
-    res = measure_device(w, n, a.steps, a.warmup, seed_rank=rank, sustain_s=a.sustain, keep=True)
+    res = measure_device(w, n, a.steps, a.warmup, seed_rank=rank, sustain_s=a.sustain, keep=True,
+                         dump_dir=a.dump_outputs if rank == 0 else None)
     if world > 1:
         dist.barrier()
     is_mul, eb, L, ctx = res['is_mul'], res['eb'], res['L'], res['ctx']
@@ -876,9 +878,8 @@ def run_gpu_arm(a, w):
     dom_name = 'k_binop<mul>' if is_mul else 'k_split'
     sec = {} if is_mul else {'recombine': dict(kernel='k_recombine', unit='GB/s', **rl['k_recombine']),
                              'step_total': dict(unit='GB/s', **rl['step_total'])}
-    traffic, traffic_src = ncu_traffic(a.workload, 'binop' if is_mul else 'split') if n == w['n'] else (None, None)
     roofline = {'bound': 'hbm', 'kernel': dom_name, 'achieved': rl[dom_name]['achieved'], 'peak': peak, 'peak_source': peak_src,
-                'unit': 'GB/s', 'frac': rl[dom_name]['frac'], 'traffic': traffic, 'traffic_source': traffic_src,
+                'unit': 'GB/s', 'frac': rl[dom_name]['frac'],
                 'ms': rl[dom_name]['ms'], 'algorithmic_bytes': rl[dom_name]['algorithmic_bytes'], **sec}
 
     gather = None
@@ -942,11 +943,7 @@ def run_gpu_arm(a, w):
             def e2e_run(count):
                 # software pipeline over successive batches: while batch j's shares are recombined (H2D-heavy), batch
                 # j+1 is split from a second host thread (D2H-heavy); the two entry points use separate workspaces in
-                # the library.  `count` splits and `count` recombinations in total.  (Measured on the B200 box with
-                # 32 MiB pipeline chunks this, the serial two-call form and the single-thread
-                # mpyc_b200_shamir_reshare_step_host were within 4 % of each other -- 41.3 / 42.4 / 44.3 ms; with
-                # call-sized chunks (128 MiB here) 37.6 / 42.3 ms: the step is bound by the PCIe throughput the
-                # chunked bidirectional copy pattern reaches, see pcie_probe.)
+                # the library.  `count` splits and `count` recombinations in total.
                 for j in range(count + 1):
                     th = None
                     if j < count:
@@ -1048,7 +1045,7 @@ def run_gpu_arm(a, w):
             'ms_per_step': ms_per_step, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': ('u8 (GF(2^8) polynomial arithmetic)' if w.get('binary') else f'u64x{L} limbs (exact integer arithmetic mod p)'), 'data': 'synthetic',
             'config': cfg, 'parallelism': f'element axis sharded over {world} GPU(s), no data-path collective',
-            'l2_policy': 'inputs (>= 1.6 GB) far larger than the 126 MB L2; no flush needed',
+            'l2_policy': 'inputs (>= 1.6 GB) far larger than the 50 MB L2; no flush needed',
             'coefficients': 'resident in HBM (parity mode)',
             'roofline': roofline, 'cpu_baseline': kind_cpu, 'e2e': e2e, 'e2e_dropin': dropin, 'small_call': small_call,
             'sustained': sustained, 'extra': extra, 'multi_selftest': selftest, 'gather': gather, 'numa': numa,
@@ -1073,7 +1070,11 @@ def main():
     ap.add_argument('--no-selftest', action='store_true', help='skip the multi-GPU pre-flight and the gather timing (N > 1)')
     ap.add_argument('--sustain', type=float, default=2.0, help='seconds of the sustained pass after the K timed steps (0 = off)')
     ap.add_argument('--config', dest='workload_alias', default=None, help='alias of --workload')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='GPU arm: write a fixed sample of the last timed step\'s outputs to DIR/<name>.npy (float64)')
     a = ap.parse_args()
+    if a.dump_outputs and a.impl != 'ours':
+        ap.error('--dump-outputs applies to the GPU arm (--impl ours)')
     if a.workload_alias:
         a.workload = a.workload_alias
     a.warmup = max(a.warmup, 3) if a.impl == 'ours' else a.warmup

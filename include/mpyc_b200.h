@@ -1,4 +1,4 @@
-/* mpyc_b200 -- C ABI of the B200 (sm_100a) batched finite-field / Shamir engine.
+/* mpyc_b200 -- C ABI of the H100 (sm_90a) batched finite-field / Shamir engine.
  *
  * The reference (lschoe/mpyc, pure Python) has no FFI; its "plugin boundary" for this path is a
  * set of Python callables that mpyc/runtime.py looks up at call time (SURVEY.md 8b).  Each entry

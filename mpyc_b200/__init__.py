@@ -1,4 +1,4 @@
-"""mpyc_b200 -- B200 (sm_100a) batched finite-field / Shamir secret-sharing engine.
+"""mpyc_b200 -- H100 (sm_90a) batched finite-field / Shamir secret-sharing engine.
 
 A from-scratch CUDA implementation of the data-parallel hot path of lschoe/mpyc
 (mpyc/thresha.py and the array half of mpyc/finfields.py), reached from Python through a thin

@@ -1,4 +1,4 @@
-"""In-tree build of libmpyc_b200.so (sm_100a) with nvcc.  No torch involved: the library is plain CUDA
+"""In-tree build of libmpyc_b200.so (sm_90a) with nvcc.  No torch involved: the library is plain CUDA
 behind a C ABI.  Objects go to mpyc_b200/csrc/_obj/, the shared library next to this file."""
 import concurrent.futures
 import hashlib
@@ -18,9 +18,9 @@ PUBLIC_HEADER = os.path.join('..', '..', 'include', 'mpyc_b200.h')
 def _headers():
     """Every header a translation unit may include: all of csrc/*.h, *.cuh plus the public C header."""
     return sorted(f for f in os.listdir(CSRC) if f.endswith(('.h', '.cuh'))) + [PUBLIC_HEADER]
-NVCC_FLAGS = ['-std=c++17', '-O3', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+NVCC_FLAGS = ['-std=c++17', '-O3', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '-Xcompiler', '-fno-strict-aliasing', '--expt-relaxed-constexpr',
-              '-Xfatbin', '-compress-all']   # compressed fatbin: the library travels to the GPU box with every gpurun call
+              '-Xfatbin', '-compress-all']   # compressed fatbin: a smaller library to load and ship
 
 
 def _nvcc():
@@ -83,7 +83,7 @@ def build(force=False, verbose=False, defines=(), lib=None):
         finally:
             OBJ, LIB = saved
     os.makedirs(OBJ, exist_ok=True)
-    stamp = LIB + '.digest'   # next to the library: travels with it to the GPU box, where nothing is rebuilt
+    stamp = LIB + '.digest'   # next to the library, so that the pair can be moved together
     digest = _digest()
 
     def fresh():

@@ -21,7 +21,7 @@ MAX_POINTS = 64
 
 
 class UnsupportedFieldError(TypeError):
-    """The modulus / shape is outside what the sm_100a kernels cover (MPYC_B200_EUNSUPPORTED)."""
+    """The modulus / shape is outside what the sm_90a kernels cover (MPYC_B200_EUNSUPPORTED)."""
 
 
 def _load():

@@ -89,8 +89,8 @@ int mpyc_grid_size(const void* kernel, size_t items, size_t dyn_smem) {
 int mpyc_sm_count() {
     int dev = 0, sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-        return 148;
-    return sms > 0 ? sms : 148;
+        return 132;
+    return sms > 0 ? sms : 132;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1342,9 +1342,8 @@ int reserve_tmp(Workspace& w, size_t bytes) {
 size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // elements per pipeline chunk, a multiple of 16: about a sixteenth of the call's traffic, at least 32 MiB and at most
-// 256 MiB per chunk.  Measured on the B200 box (C3 shape, n = 2^24, split of batch j+1 concurrent with the recombination
-// of batch j): 8 MiB chunks 48.5 ms per step, 32 MiB 40.4 ms, 128 MiB 35.2 ms -- many small 2-D copies in both
-// directions leave PCIe below what two large concurrent copies reach.  MPYC_B200_CHUNK_MB overrides (tuning).
+// 256 MiB per chunk: many small 2-D copies in both directions leave PCIe below what two large concurrent copies
+// reach.  MPYC_B200_CHUNK_MB overrides (tuning).
 size_t chunk_elems(size_t n, size_t bytes_per_elem_total) {
     static const size_t forced = [] {
         const char* e = getenv("MPYC_B200_CHUNK_MB");

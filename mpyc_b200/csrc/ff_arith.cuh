@@ -1,4 +1,4 @@
-// Multi-limb prime-field arithmetic for sm_100a (and, for table preparation and algorithm
+// Multi-limb prime-field arithmetic for sm_90a (and, for table preparation and algorithm
 // tests, the host).  Elements are L little-endian 64-bit limbs in memory (L in {1,2,3,4}); in
 // registers they are handled as N = 2L 32-bit limbs, because the native multiplier is
 // IMAD.WIDE.U32 (32x32+64 with carry in/out): every mad.lo.cc.u32 / madc.hi.cc.u32 pair below is

@@ -1,6 +1,6 @@
-// sm_100a kernels for the GF(p) Shamir hot path.  All kernels are persistent grid-stride
-// streamers: one CTA wave sized from the SM count, 256-bit global loads/stores on the limb
-// arrays (LDG.E.256 / STG.E.256; read-once data bypasses L1 allocation), per-call constant tables
+// sm_90a kernels for the GF(p) Shamir hot path.  All kernels are persistent grid-stride
+// streamers: one CTA wave sized from the SM count, 128-bit global loads/stores on the limb
+// arrays (LDG.E.128 / STG.E.128; read-once data bypasses L1 allocation), per-call constant tables
 // (Vandermonde / Lagrange, a few hundred bytes) staged global -> shared memory once per CTA with a
 // TMA bulk copy (cp.async.bulk + mbarrier; UBLKCP in SASS); K4 also stages its PRF byte tiles that
 // way, double-buffered.  Integer modular work: no tensor cores.
@@ -71,33 +71,15 @@ __device__ __forceinline__ void stg_v2(u64* p, const u32* v) {
     asm volatile("st.global.L1::no_allocate.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(v[0]), "r"(v[1]) : "memory");
 }
 
-__device__ __forceinline__ void ldg_v8(u32* v, const u64* p) {   // 32 bytes = four 64-bit limbs (LDG.E.256)
-    asm("ld.global.nc.L1::no_allocate.v8.u32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "l"(p));
-}
-__device__ __forceinline__ void stg_v8(u64* p, const u32* v) {
-    asm volatile("st.global.L1::no_allocate.v8.u32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]),
-                 "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-
-// load / store NL 64-bit limbs starting at p, as 2*NL 32-bit registers.  VEC: 256-bit accesses
-// (sm_100 LDG.E.256 / STG.E.256; p 32-byte aligned, NL a multiple of 4); else one limb at a time.
-#ifndef MPYC_VEC128
-#define MPYC_VEC128 0   // 1: split every 256-bit access into two 128-bit ones (experiments)
-#endif
+// load / store NL 64-bit limbs starting at p, as 2*NL 32-bit registers.  VEC: 128-bit accesses, the widest
+// global access sm_90 has (LDG.E.128 / STG.E.128), in pairs covering 32-byte groups (p 32-byte aligned, NL a
+// multiple of 4); else one limb at a time.
 template <int NL, bool VEC>
 __device__ __forceinline__ void load_limbs(u32* v, const u64* p) {
     if constexpr (VEC) {
         static_assert(NL % 4 == 0, "vector path moves 32-byte groups");
 #pragma unroll
-        for (int q = 0; q < NL / 4; q++) {
-            if constexpr (MPYC_VEC128) {
-                ldg_v4(v + 8 * q, p + 4 * q);
-                ldg_v4(v + 8 * q + 4, p + 4 * q + 2);
-            } else {
-                ldg_v8(v + 8 * q, p + 4 * q);
-            }
-        }
+        for (int q = 0; q < NL / 2; q++) ldg_v4(v + 4 * q, p + 2 * q);
     } else {
 #pragma unroll
         for (int q = 0; q < NL; q++) ldg_v2(v + 2 * q, p + q);
@@ -107,14 +89,7 @@ template <int NL, bool VEC>
 __device__ __forceinline__ void store_limbs(u64* p, const u32* v) {
     if constexpr (VEC) {
 #pragma unroll
-        for (int q = 0; q < NL / 4; q++) {
-            if constexpr (MPYC_VEC128) {
-                stg_v4(p + 4 * q, v + 8 * q);
-                stg_v4(p + 4 * q + 2, v + 8 * q + 4);
-            } else {
-                stg_v8(p + 4 * q, v + 8 * q);
-            }
-        }
+        for (int q = 0; q < NL / 2; q++) stg_v4(p + 2 * q, v + 4 * q);
     } else {
 #pragma unroll
         for (int q = 0; q < NL; q++) stg_v2(p + q, v + 2 * q);
@@ -335,15 +310,13 @@ k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, in
 //   full : table entry is a full field element in table form; acc (2L+1 limbs), one reduction
 // ---------------------------------------------------------------------------------------
 
-// items in flight per thread (tuned on B200: split is fastest without unrolling, recombine with
-// 4 items for 1-limb and 2 items for 2-limb fields); override with -D for experiments
+// items in flight per thread (split is fastest without unrolling, recombine with 4 items for 1-limb and 2 items
+// for 2-limb fields); override with -D for experiments
 #ifndef MPYC_SPLIT_U
 #define MPYC_SPLIT_U 1
 #endif
-// shares computed per trip of the party loop of split_compute: two independent share evaluations in flight
-// hide the carry-chain latency for fields of >= 2 limbs (measured on B200, C3: K2 0.87 -> 0.955 of the copy
-// peak, C5 shape 0.87 -> 0.94); 1-limb fields (0.874 vs 0.852) and the Barrett path of generic primes
-// (0.739 vs 0.677) are fastest without
+// shares computed per trip of the party loop of split_compute: two independent share evaluations in flight, one
+// share's carry chains issuing while the other's wait.  Neutral on an H100 SXM at 400 W (DESIGN.md section 5)
 #ifndef MPYC_SPLIT_MU
 #define MPYC_SPLIT_MU ((L == 1 || KIND == KIND_GENERIC) ? 1 : 2)
 #endif
@@ -410,8 +383,7 @@ __device__ __forceinline__ void split_items(const FieldParams& f, const u64* sec
 }
 
 #ifndef MPYC_SPLIT_PREFETCH
-// software-pipelined main loop of k_split for fields of at most this many limbs (0 = off).  Measured on B200, ns64
-// (1 limb, 160 bytes per thread and trip, long-scoreboard bound at 46 % warps active): K2 0.874 -> 0.937 of the copy peak
+// software-pipelined main loop of k_split for fields of at most this many limbs (0 = off; neutral on an H100 SXM)
 #define MPYC_SPLIT_PREFETCH 1
 #endif
 #ifndef MPYC_SPLIT_MINB
@@ -703,9 +675,8 @@ __device__ __forceinline__ void recombine_items_small(const FieldParams& f, cons
 }
 
 #ifndef MPYC_RECS_MINB1
-// min resident CTAs per SM for the small-lambda recombination of 1-limb fields.  Measured on B200 (ns64, k = 2): the
-// kernel compiles to 88 registers = 2 CTAs/SM and runs at 0.71 of the copy peak; capped at 4 CTAs/SM (64 registers)
-// 0.92 -- the full-product form it replaces (121 registers) does 0.895; 3 CTAs/SM 0.84
+// min resident CTAs per SM for the small-lambda recombination of 1-limb fields: 4 (64 registers) instead of the 2
+// its 88 registers allow (3 % faster on an H100 SXM, DESIGN.md section 5)
 #define MPYC_RECS_MINB1 4
 #endif
 template <int L, int KIND, bool VEC>

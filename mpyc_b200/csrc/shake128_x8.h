@@ -1,8 +1,8 @@
 // Eight SHAKE128 sponges advancing in lock step on one core: Keccak-f[1600] on 8 independent states held lane-interleaved
 // in 25 zmm registers (AVX-512F: vprolq for rho, vpternlogq for theta's three-way xor and for chi).  One sponge is
 // strictly sequential, but a PRSS call squeezes C(m-1, t) of them -- one per key subset (thresha.py:257) -- and when
-// the host has fewer cores than subsets (the 8-vCPU GPU box of round 1: 20 subsets for m = 7, t = 3) each worker
-// thread owns several: x8 squeezes them together at ~4.8x the scalar sponge's rate per core.
+// the host has fewer cores than subsets (20 subsets for m = 7, t = 3 on an 8-vCPU host) each worker
+// thread owns several: x8 squeezes them together.
 // All sponges of a group absorb messages of the SAME length (key || uci) and are squeezed by the same amounts.
 #pragma once
 #include <stddef.h>

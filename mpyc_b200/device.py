@@ -26,7 +26,7 @@ def _require_cuda():
 
 def _alloc(ctx, rows, n, device):
     """Uninitialised limb storage: int64 (rows, n, L) or uint8 (rows, n); row stride padded to 32 bytes
-    so that every row start allows 256-bit vector accesses."""
+    so that every row start allows the 32-byte vector path."""
     _require_cuda()
     if ctx.binary:
         stride = (n + 31) // 32 * 32

@@ -116,7 +116,7 @@ class PeerReshare:
         if len(set(self.dealers)) != len(self.dealers) or m > 32:
             raise ValueError('peer resharing needs 2t+1 <= m <= 32')
         L = ctx.nlimbs
-        self.row_bytes = (n * L * 8 + 31) // 32 * 32            # rows 32-byte aligned (256-bit stores)
+        self.row_bytes = (n * L * 8 + 31) // 32 * 32            # rows 32-byte aligned (32-byte store groups)
         self.slots = max(len(local_parties(m, self.world, r)) for r in range(self.world))
         nbytes = 2 * self.slots * len(self.dealers) * self.row_bytes
         # own receive buffer: [generation][local party slot][dealer index] rows, exported to the other ranks

@@ -1,4 +1,4 @@
-"""install(): put the B200 engine behind an imported MPyC without touching MPyC's code.
+"""install(): put the GPU engine behind an imported MPyC without touching MPyC's code.
 
 mpyc/runtime.py looks the secret-sharing functions up as attributes of the `mpyc.thresha` module at
 call time (runtime.py:478-485,565-572,647-656,963,982,1280,4057,4099,4219,4248); assigning the drop-in

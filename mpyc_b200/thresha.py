@@ -1,4 +1,4 @@
-"""Drop-in replacements for the reference's secret-sharing module, backed by the sm_100a engine.
+"""Drop-in replacements for the reference's secret-sharing module, backed by the sm_90a engine.
 
 Same names, argument meaning, return types and error behaviour as mpyc/thresha.py:
     random_split :23, np_random_split :47, _recombination_vector :67, recombine :88,

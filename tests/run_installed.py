@@ -1,5 +1,5 @@
 """Launcher: run an UNMODIFIED MPyC program (a demo of the reference, or any script using `from mpyc.runtime import mpc`)
-with the B200 engine installed behind mpyc.thresha / mpyc.finfields.
+with the GPU engine installed behind mpyc.thresha / mpyc.finfields.
 
     python tests/run_installed.py <program.py> [program and MPyC flags, e.g. -M3 -1]
 

@@ -25,7 +25,7 @@ def checker():
     hdr = os.path.join(HERE, '..', 'mpyc_b200', 'csrc', 'ff_arith.cuh')
     if not os.path.exists(BIN) or os.path.getmtime(BIN) < max(os.path.getmtime(SRC), os.path.getmtime(hdr)):
         os.makedirs(os.path.dirname(BIN), exist_ok=True)
-        subprocess.run([nvcc, '-std=c++17', '-O3', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', BIN, SRC], check=True)
+        subprocess.run([nvcc, '-std=c++17', '-O3', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', BIN, SRC], check=True)
 
     def run(lines):
         r = subprocess.run([BIN], input='\n'.join(lines) + '\n', capture_output=True, text=True, check=True)

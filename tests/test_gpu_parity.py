@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle and the golden fixtures
-generated from the real reference.  Bit-exact everywhere (integer work).  Run on the B200 box:
+generated from the real reference.  Bit-exact everywhere (integer work).  Run on an H100:
     python -m pytest tests -m gpu -x -q
 """
 import itertools
@@ -536,7 +536,7 @@ def test_batched_inverse_montgomery_trick(p, batch, monkeypatch):
 
 
 def test_batched_inverse_large_property():
-    """n = 2^21 (the launcher picks batch 8 on a 148-SM part): a * a^-1 == 1 everywhere, checked on the device."""
+    """n = 2^21 (the launcher picks batch 8 on a 132-SM H100): a * a^-1 == 1 everywhere, checked on the device."""
     for p in (2**128 - 173, 9409569905028393239):
         ctx = mpyc_b200.context_for(p)
         n = (1 << 21) + 5

@@ -1,14 +1,15 @@
-"""install() against the REAL reference (only where /root/reference exists, i.e. the build container):
+"""install() against the REAL reference (only where it is available, see oracle/reference.py):
 attribute swap, pass-through for fields the engine does not cover, host-only helpers equal to the
 reference's, and no silent CPU computation for covered fields."""
-import os
 import sys
 
 import pytest
 
-REF = os.environ.get('MPYC_REFERENCE', '/root/reference')
-if not os.path.isdir(os.path.join(REF, 'mpyc')):
-    pytest.skip('reference checkout not present', allow_module_level=True)
+from oracle import reference
+
+REF = reference.path()
+if REF is None:
+    pytest.skip('reference not present ($MPYC_REFERENCE, or the copy build() makes in oracle/_ref)', allow_module_level=True)
 
 
 @pytest.fixture(scope='module')

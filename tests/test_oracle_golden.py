@@ -3,16 +3,20 @@
 Every function of the oracle is replayed on the inputs stored in tests/golden/*.json and must
 reproduce the reference's outputs bit for bit.  Runs on CPU (no GPU, no reference needed).
 """
+from collections import defaultdict
+
 import pytest
 
+import random_instances as ri
 from oracle import shamir_oracle as orc
-from golden_util import load, unhex
+from golden_util import digest, load, unhex
 
 SPLIT = load('split_recombine.json')
 PRF = load('prf.json')
 PRSS = load('prss.json')
 FF = load('finfields.json')
 G256 = load('gf256.json')
+RANDOM = load('random_instances.json')   # digests of the reference's results on tests/random_instances.py's instances
 
 
 def test_default_primes_match_reference_find_prime_root():
@@ -216,3 +220,58 @@ def test_local_conv2d(case):
     p = int(case['p'], 16)
     k, r, m, n, v, s = case['shape']
     assert orc.local_conv2d(p, unhex(case['X']), unhex(case['W']), unhex(case['B']), k, r, m, n, v, s) == unhex(case['Y'])
+
+
+def _check_random(test, p, results):
+    want = dict(zip(ri.KINDS[test], RANDOM[test][ri.PRIMES.index(p)]))
+    assert {k: digest(results[k]) for k in want} == want
+
+
+@pytest.mark.parametrize('p', ri.PRIMES, ids=lambda p: f'p{p.bit_length()}')
+def test_split_recombine_prss_random_instances(p):
+    Fo = orc.field_of(p)
+    got = defaultdict(list)
+    for c in ri.split_instances(p):
+        m, t, n, s, stream, xs, i, keys, uci = (c[k] for k in ('m', 't', 'n', 's', 'stream', 'xs', 'i', 'keys', 'uci'))
+        sh_np = orc.split_np_order(Fo, s, orc.np_stream_to_C(stream, t, n), m)
+        rec = orc.recombine(Fo, xs, [sh_np[x - 1] for x in xs])
+        assert rec == s
+        got['shares_np'].append(sh_np)
+        got['shares_list'].append(orc.split_list_order(Fo, s, orc.list_stream_to_c(stream, t, n), m))
+        got['recombination_vectors'].append([orc.recombination_vector(Fo, xs, x_r) for x_r in (0, m + 1)])
+        got['recombined'].append(rec)
+        got['f_S_i'].append([orc.f_S_i(Fo, m, i, S) % p for S in keys])
+        got['prss'].append(orc.prss_share(Fo, m, i, {S: orc.prf_values(k, p, uci, n) for S, k in keys.items()}, n))
+        if t:
+            prl = {S: orc.prf_values(k, p, uci, n * t) for S, k in keys.items()}
+            got['prss_zero_np'].append(orc.prss_share_zero_np_order(Fo, m, i, prl, n))
+            got['prss_zero_list'].append(orc.prss_share_zero_list_order(Fo, m, i, prl, n))
+    _check_random('split', p, got)
+
+
+@pytest.mark.parametrize('p', ri.PRIMES, ids=lambda p: f'p{p.bit_length()}')
+def test_field_array_operators_random_instances(p):
+    a, b = ri.operator_instance(p)
+    got = {'add': orc.ff_add(p, a, b), 'sub': orc.ff_sub(p, a, b), 'mul': orc.ff_mul(p, a, b), 'neg': orc.ff_neg(p, a),
+           'inv': orc.ff_inv(p, b), 'div': orc.ff_div(p, a, b), 'lshift5': orc.ff_lshift(p, a, 5),
+           'rshift5': orc.ff_rshift(p, a, 5), 'pow7': orc.ff_pow(p, a, 7)}
+    _check_random('operators', p, got)
+
+
+@pytest.mark.parametrize('p', ri.PRIMES, ids=lambda p: f'p{p.bit_length()}')
+def test_local_algebra_random_instances(p):
+    """oracle.local_* against the expressions of np_random_bits / np_trunc / np_sgn / np_to_bits (mpyc/runtime.py:860,
+    870, 3646-3660, 4252-4271, 4415) evaluated on the reference's field arrays, random sizes and bit counts."""
+    got = defaultdict(list)
+    for c in ri.local_instances(p):
+        n, f, a, b, cc, bits, ln = (c[k] for k in ('n', 'f', 'a', 'b', 'c', 'bits', 'l'))
+        got['square_add'].append(orc.local_fma(p, a, a, cc))
+        got['mul_add'].append(orc.local_fma(p, a, b, cc))
+        got['axpb'].append(orc.local_axpb(p, a, c['s'], c['t']))
+        got['low_bits'].append(orc.local_low_bits(cc, c['nb']))
+        got['nonzero'].append(orc.local_nonzero(a))
+        got['compose_ascending'].append(orc.local_bits_compose(p, bits, n, f))
+        got['compose_descending'].append(orc.local_bits_compose(p, bits, n, f, descending=True))
+        got['decompose_descending'].append(orc.local_bits_decompose(cc, ln, descending=True))
+        got['decompose_ascending'].append(orc.local_bits_decompose(cc, ln))
+    _check_random('local', p, got)

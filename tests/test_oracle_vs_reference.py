@@ -1,17 +1,19 @@
-"""Live cross-check of the oracle against the UNMODIFIED reference (only where /root/reference exists, i.e. the build
-container): beyond the committed golden fixtures, randomised (p, m, t, n) instances of every function on the path --
-split (np and list order), recombination vectors and recombination, f_S(i), PRF, PRSS shares and zero-shares, and the
-field-array operators -- with secrets.randbelow replaced by a fixed stream for the duration of each reference call."""
+"""Live cross-check of the oracle against the UNMODIFIED reference where it is available (oracle/reference.py):
+randomised (p, m, t, n) instances of every function on the path -- split (np and list order), recombination vectors and
+recombination, f_S(i), PRF, PRSS shares and zero-shares, and the field-array operators -- with secrets.randbelow
+replaced by a fixed stream for the duration of each reference call.  tests/test_oracle_golden.py replays stored digests
+of the reference's results on the same instances (tests/random_instances.py) where it is not."""
 import itertools
-import os
 import random
 import sys
 
 import pytest
 
-REF = os.environ.get('MPYC_REFERENCE', '/root/reference')
-if not os.path.isdir(os.path.join(REF, 'mpyc')):
-    pytest.skip('reference checkout not present', allow_module_level=True)
+from oracle import reference
+
+REF = reference.path()
+if REF is None:
+    pytest.skip('reference not present ($MPYC_REFERENCE, or the copy build() makes in oracle/_ref)', allow_module_level=True)
 
 from oracle import shamir_oracle as orc   # noqa: E402
 

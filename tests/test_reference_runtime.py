@@ -3,12 +3,10 @@ own unittest files) running on top of mpyc_b200.install().
 
 Two device modes, same tests:
   * 'oracle'  (build container, no GPU; not gpu-marked): the four device round trips of mpyc_b200.thresha are answered
-    by tests/oracle_device.py, everything above them is the product code.  Needs the reference checkout
-    (/root/reference or $MPYC_REFERENCE); skipped where it is absent.
-  * 'cuda'    (-m gpu): the real kernels through the C ABI.  On the GPU box the reference is importable from
-    baseline/_ref (pip install --target of the unmodified checkout plus its demos/ and tests/ under _checkout/,
-    git-ignored, written by tools/install_reference.sh) or $MPYC_REFERENCE; tests that need the reference's tests/
-    or demos/ directories skip when only the package is there.
+    by tests/oracle_device.py, everything above them is the product code.
+  * 'cuda'    (-m gpu): the real kernels through the C ABI.
+Both need the reference: $MPYC_REFERENCE, or the copy of it that build() makes in oracle/_ref/ (oracle/reference.py);
+they skip where it is absent.
 
 Every run goes through tests/run_installed.py in a child process (MPyC parses sys.argv and builds its runtime at import;
 -M3 re-executes the command line for the other parties, mpyc/runtime.py:5156-5189).
@@ -23,29 +21,21 @@ import sys
 
 import pytest
 
+from oracle import reference
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 LAUNCHER = os.path.join(HERE, 'run_installed.py')
 PROGRAM = os.path.join(HERE, 'programs', 'secure_ops.py')
 FIPS197 = '69c4e0d86a7b0430d8cdb78070b4c55a'
 
 
-def _find_reference():
-    for cand in (os.environ.get('MPYC_REFERENCE'), '/root/reference', os.path.join(ROOT, 'baseline', '_ref')):
-        if cand and os.path.isdir(os.path.join(cand, 'mpyc')):
-            return cand
-    return None
-
-
-REF = _find_reference()
+REF = reference.path()
 
 
 def _checkout_dir(name):
-    """The reference's tests/ or demos/ directory: in the checkout, or next to a package-only install
-    (baseline/_ref/_checkout, written by tools/install_reference.sh)."""
-    for base in (REF, os.path.join(REF or '', '_checkout')):
-        if base and os.path.isdir(os.path.join(base, name)):
-            return os.path.join(base, name)
+    """The reference's tests/ or demos/ directory, where the reference copy has it."""
+    if REF and os.path.isdir(os.path.join(REF, name)):
+        return os.path.join(REF, name)
     return None
 
 
@@ -67,7 +57,7 @@ def _has_cuda():
 @pytest.fixture(params=['oracle', pytest.param('cuda', marks=pytest.mark.gpu)])
 def mode(request):
     if REF is None:
-        pytest.skip('no reference available (MPYC_REFERENCE, /root/reference or baseline/_ref)')
+        pytest.skip('no reference available ($MPYC_REFERENCE or the copy build() makes in oracle/_ref)')
     if request.param == 'cuda' and not _has_cuda():
         pytest.skip('no CUDA device')
     if request.param == 'oracle' and _has_cuda():

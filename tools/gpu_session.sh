@@ -20,7 +20,7 @@ set -u
 OUT=gpurun_out
 mkdir -p $OUT
 export PYTHONDONTWRITEBYTECODE=1
-REFDIR=$PWD/baseline/_ref
+REFDIR=$PWD/oracle/_ref        # build() with MPYC_REFERENCE set (oracle/reference.py)
 launcher() { MPYC_REFERENCE=$REFDIR python tests/run_installed.py "$@"; }
 
 for step in "$@"; do

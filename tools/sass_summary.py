@@ -54,12 +54,12 @@ def main():
             def cnt(rx):
                 return sum(1 for i in ins if re.match(rx, i))
             reg, stack, shared, local = usage.get(name, (None, None, None, None))
-            rows.append((dem, len(ins), cnt(r'UBLKCP'), cnt(r'LDG\.E.*\.256|LDG.*256'), cnt(r'STG\.E.*\.256|STG.*256'), cnt(r'LDG'), cnt(r'STG'),
+            rows.append((dem, len(ins), cnt(r'UBLKCP'), cnt(r'LDG\.E.*\.128'), cnt(r'STG\.E.*\.128'), cnt(r'LDG'), cnt(r'STG'),
                          cnt(r'IMAD\.WIDE'), cnt(r'IMAD'), cnt(r'IADD3|IADD'), cnt(r'LOP3|SHF|SEL'), cnt(r'LDS|STS'), cnt(r'LDGSTS'),
                          cnt(r'HMMA|IMMA|UTCMMA|UTMALDG'), reg, stack, local, shared))
-    hdr = ('kernel', 'SASS', 'UBLKCP', 'LDG256', 'STG256', 'LDG', 'STG', 'IMAD.W', 'IMAD*', 'IADD3', 'LOP/SHF/SEL', 'LDS/STS', 'LDGSTS', 'tensor', 'regs',
+    hdr = ('kernel', 'SASS', 'UBLKCP', 'LDG128', 'STG128', 'LDG', 'STG', 'IMAD.W', 'IMAD*', 'IADD3', 'LOP/SHF/SEL', 'LDS/STS', 'LDGSTS', 'tensor', 'regs',
            'stack', 'local', 'smem')
-    print('# static SASS / resource summary of the hot kernels (sm_100a), tools/sass_summary.py')
+    print('# static SASS / resource summary of the hot kernels (sm_90a), tools/sass_summary.py')
     print(('%-44s' + ' %7s' * (len(hdr) - 1)) % hdr)
     for r in sorted(rows):
         print(('%-44s' + ' %7s' * (len(r) - 1)) % r)

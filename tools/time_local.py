@@ -14,7 +14,7 @@ import mpyc_b200   # noqa: E402
 from mpyc_b200 import device as dev   # noqa: E402
 from mpyc_b200.device import DeviceArray   # noqa: E402
 
-PEAK = 6568.7
+PEAK = 3350.0   # H100 SXM data sheet (HBM3), unless MEASURED_PEAKS.json gives a measured one
 try:
     with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'MEASURED_PEAKS.json')) as fh:
         peaks = json.load(fh)
