@@ -17,6 +17,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <type_traits>
 #include <vector>
 
@@ -61,13 +62,13 @@ static int fail(int code, const char* msg) {
 
 int mpyc_grid_size(const void* kernel, size_t items, size_t dyn_smem) {
     static std::mutex mu;
-    static std::map<std::pair<const void*, int>, int> wave;   // (kernel, device) -> CTAs per full wave
+    static std::map<std::tuple<const void*, int, size_t>, int> wave;   // (kernel, device, dynamic smem) -> CTAs per full wave
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return -1;
     int w;
     {
         std::lock_guard<std::mutex> g(mu);
-        auto key = std::make_pair(kernel, dev);
+        auto key = std::make_tuple(kernel, dev, dyn_smem);
         auto it = wave.find(key);
         if (it == wave.end()) {
             int sms = 0, occ = 0;

@@ -8,7 +8,8 @@
 //   K1   k_binop                                finfields.py:1056-1124,1189-1192
 //   K1b  k_pow (pow / sqrt / is_sqr), k_inv_batch (Montgomery-trick inverse)   finfields.py:1408-1470
 //   K1c  k_matmul                               finfields.py:1126-1146
-//   K2   k_split (small / full tables), k_split_gen (ChaCha20 coefficients, strided or per-row destinations),
+//   K2   k_split_tiled (aligned rows; shares leave through shared memory as TMA bulk stores), k_split (small / full
+//        tables; unaligned rows and 3-limb fields), k_split_gen (ChaCha20 coefficients, strided or per-row destinations),
 //        k_split_dyn (any t)                    thresha.py:47-64
 //   K3   k_recombine, k_recombine_small         thresha.py:119-132
 //   K4   k_prss_tiles, k_prss_combine           thresha.py:163-173,201-217
@@ -330,6 +331,47 @@ k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, in
 #define MPYC_RECS_U 1
 #endif
 
+// Tiled K2 (k_split_tiled): a CTA owns a tile of MPYC_THREADS x 32 bytes of every row (8 KB).  A thread's item is two
+// 16-byte chunks at tile limb offsets o and o + H: for L <= 2 the chunks tid and tid + MPYC_THREADS, so that a warp
+// load covers 512 contiguous bytes; for L = 4 the two halves of element tid.
+#define MPYC_TILE_LIMBS (MPYC_THREADS * 4)
+template <int L>
+struct TileItem {
+    static constexpr int STEP = (L == 4) ? 4 : 2;                      // o = STEP * tid
+    static constexpr int H = (L == 4) ? 2 : 2 * MPYC_THREADS;          // limbs from the first chunk to the second
+};
+// share rows written a tile item at a time; SMEM: the tile's stage in shared memory (stride MPYC_TILE_LIMBS), each row
+// at the same offsets as in its global row
+template <int L, bool SMEM>
+struct TileDst {
+    u64* base;
+    size_t stride;
+    __device__ __forceinline__ u64* row(int i) const { return base + (size_t)i * stride; }
+};
+
+template <int L>
+__device__ __forceinline__ void load_tile_item(u32* v, const u64* p) {
+    ldg_v4(v, p);
+    ldg_v4(v + 4, p + TileItem<L>::H);
+}
+
+template <int NL, bool VEC, class DST>
+__device__ __forceinline__ void store_share(const DST& dst, int i, size_t limb_off, const u32* r) {
+    store_limbs<NL, VEC>(dst.row(i) + limb_off, r);
+}
+template <int NL, bool VEC, int L, bool SMEM>
+__device__ __forceinline__ void store_share(const TileDst<L, SMEM>& dst, int i, size_t limb_off, const u32* r) {
+    static_assert(NL == 4, "a tile item is two 16-byte chunks");
+    u64* p = dst.row(i) + limb_off;
+    if constexpr (SMEM) {
+        *reinterpret_cast<uint4*>(p) = make_uint4(r[0], r[1], r[2], r[3]);
+        *reinterpret_cast<uint4*>(p + TileItem<L>::H) = make_uint4(r[4], r[5], r[6], r[7]);
+    } else {
+        stg_v4(p, r);
+        stg_v4(p + TileItem<L>::H, r + 4);
+    }
+}
+
 // shares of one item (E elements) from its t+1 polynomial coefficient rows held in registers
 template <int L, int KIND, int TP1, bool FULL, int E, bool VEC, class DST>
 __device__ __forceinline__ void split_compute(const FieldParams& f, const u32 (*M)[E * 2 * L], const DST& dst,
@@ -358,7 +400,7 @@ __device__ __forceinline__ void split_compute(const FieldParams& f, const u32 (*
                 else copy_n<N>(r + e * N, acc);
             }
         }
-        store_limbs<E * L, VEC>(dst.row(i) + limb_off, r);
+        store_share<E * L, VEC>(dst, i, limb_off, r);
     }
 }
 
@@ -392,7 +434,7 @@ __device__ __forceinline__ void split_items(const FieldParams& f, const u64* sec
 #ifndef MPYC_SPLIT_MINB1
 #define MPYC_SPLIT_MINB1 1  // the same for 1-limb fields with t+1 <= 2 (ns64: 52 registers miss the 5th CTA per SM by one)
 #endif
-template <int L, int KIND, int TP1, bool FULL, bool VEC>
+template <int L, int KIND, int TP1, bool FULL>
 __global__ void __launch_bounds__(MPYC_THREADS, (L == 1 && TP1 <= 2 && !FULL) ? MPYC_SPLIT_MINB1 : MPYC_SPLIT_MINB)
 k_split(FieldParams f, const u64* __restrict__ secrets, const u64* __restrict__ coeffs, size_t cstride,
         u64* __restrict__ shares, size_t sstride, size_t n, int m, const u64* __restrict__ gtab, u32 tab_bytes) {
@@ -400,48 +442,112 @@ k_split(FieldParams f, const u64* __restrict__ secrets, const u64* __restrict__ 
     extern __shared__ __align__(16) u64 stab[];
     __shared__ __align__(8) u64 mbar;
     tma_stage_table(stab, gtab, tab_bytes, &mbar);
-    constexpr int E = VEC ? VecItem<L>::E : 1;
     constexpr int U = (TP1 * L <= 8) ? MPYC_SPLIT_U : 1;
     const size_t nth = (size_t)gridDim.x * blockDim.x;
-    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t n_items = n / E;
-    size_t it = tid;
+    size_t it = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if constexpr (L <= MPYC_SPLIT_PREFETCH && !FULL && TP1 <= 3) {
         // software pipeline for the narrow fields (few bytes per item, latency-bound at one item per trip): the t+1
         // input vectors of item it+nth are requested before the shares of item it are computed and stored
         constexpr int N = 2 * L;
-        u32 cur[TP1][E * N], nxt[TP1][E * N];
-        auto fetch = [&](u32 (*M)[E * N], size_t item) {
-            const size_t off = item * (size_t)(E * L);
-            load_limbs<E * L, VEC>(M[0], secrets + off);
+        u32 cur[TP1][N], nxt[TP1][N];
+        auto fetch = [&](u32 (*M)[N], size_t item) {
+            const size_t off = item * (size_t)L;
+            load_limbs<L, false>(M[0], secrets + off);
 #pragma unroll
-            for (int j = 1; j < TP1; j++) load_limbs<E * L, VEC>(M[j], coeffs + (size_t)(j - 1) * cstride + off);
+            for (int j = 1; j < TP1; j++) load_limbs<L, false>(M[j], coeffs + (size_t)(j - 1) * cstride + off);
         };
-        if (it < n_items) fetch(cur, it);
-        for (; it < n_items; it += nth) {
-            const bool more = it + nth < n_items;
+        if (it < n) fetch(cur, it);
+        for (; it < n; it += nth) {
+            const bool more = it + nth < n;
             if (more) fetch(nxt, it + nth);
-            split_compute<L, KIND, TP1, FULL, E, VEC>(f, cur, dst, m, stab, it * (size_t)(E * L));
+            split_compute<L, KIND, TP1, FULL, 1, false>(f, cur, dst, m, stab, it * (size_t)L);
             if (more) {
 #pragma unroll
                 for (int j = 0; j < TP1; j++)
 #pragma unroll
-                    for (int q = 0; q < E * N; q++) cur[j][q] = nxt[j][q];
+                    for (int q = 0; q < N; q++) cur[j][q] = nxt[j][q];
             }
         }
     } else {
-        for (; it + (U - 1) * nth < n_items; it += U * nth)
-            split_items<L, KIND, TP1, FULL, E, VEC, U>(f, secrets, coeffs, cstride, dst, m, stab,
-                                                       it * (size_t)(E * L), nth * (size_t)(E * L));
-        for (; it < n_items; it += nth)
-            split_items<L, KIND, TP1, FULL, E, VEC, 1>(f, secrets, coeffs, cstride, dst, m, stab,
-                                                       it * (size_t)(E * L), 0);
+        for (; it + (U - 1) * nth < n; it += U * nth)
+            split_items<L, KIND, TP1, FULL, 1, false, U>(f, secrets, coeffs, cstride, dst, m, stab, it * (size_t)L,
+                                                         nth * (size_t)L);
+        for (; it < n; it += nth)
+            split_items<L, KIND, TP1, FULL, 1, false, 1>(f, secrets, coeffs, cstride, dst, m, stab, it * (size_t)L, 0);
     }
-    if constexpr (E > 1) {
-        for (size_t h = n_items * E + tid; h < n; h += nth)
-            split_items<L, KIND, TP1, FULL, 1, false, 1>(f, secrets, coeffs, cstride, dst, m, stab,
-                                                         h * (size_t)L, 0);
+}
+
+// K2 for 32-byte aligned rows of 1-, 2- and 4-limb fields, one tile (TileItem) per CTA and trip.  STAGE: the shares are
+// written to a stage of m x 8 KB in shared memory at their tile offsets and leave as one TMA bulk store per row
+// (cp.async.bulk, UBLKCP in SASS); otherwise (m too large for the stage) every thread stores its two chunks itself
+// (coalesced for L <= 2).  Whole sectors instead of a 32-byte item per thread, which used half of every sector a warp
+// access touched (a 3 in / 5 out stream probe: 2235 -> 2822 GB/s on an H100 SXM at 400 W, DESIGN.md section 5).
+// For t+1 <= 4 the input chunks of the thread's next tile are requested before the current tile's shares are computed.
+// smem layout: [table (tab_bytes rounded up to 128)] [stage: m x MPYC_TILE_LIMBS limbs]
+template <int L, int KIND, int TP1, bool FULL, bool STAGE>
+__global__ void MPYC_LB
+k_split_tiled(FieldParams f, const u64* __restrict__ secrets, const u64* __restrict__ coeffs, size_t cstride,
+              u64* __restrict__ shares, size_t sstride, size_t n, int m, const u64* __restrict__ gtab, u32 tab_bytes) {
+    extern __shared__ __align__(128) u64 smem[];
+    __shared__ __align__(8) u64 mbar;
+    tma_stage_table(smem, gtab, tab_bytes, &mbar);
+    constexpr int E = VecItem<L>::E, N = 2 * L;
+    constexpr int TE = MPYC_TILE_LIMBS / L;   // elements per tile
+    const size_t ntiles = n / TE;
+    const u32 o = threadIdx.x * TileItem<L>::STEP;
+    u64* const stage = smem + ((tab_bytes + 127u) & ~127u) / sizeof(u64);
+    u32 cur[TP1][E * N], nxt[TP1][E * N];
+    auto fetch = [&](u32 (*M)[E * N], size_t tile) {
+        const size_t off = tile * MPYC_TILE_LIMBS + o;
+        load_tile_item<L>(M[0], secrets + off);
+#pragma unroll
+        for (int j = 1; j < TP1; j++) load_tile_item<L>(M[j], coeffs + (size_t)(j - 1) * cstride + off);
+    };
+    // more coefficient rows held for the next tile cost more occupancy than they hide (64-bit m = 17, t = 8: 172 registers)
+    constexpr bool PREFETCH = TP1 <= 4;
+    size_t tile = blockIdx.x;
+    if (PREFETCH && tile < ntiles) fetch(cur, tile);
+    for (; tile < ntiles; tile += gridDim.x) {
+        const bool more = PREFETCH && tile + gridDim.x < ntiles;
+        if constexpr (PREFETCH) {
+            if (more) fetch(nxt, tile + gridDim.x);
+        } else {
+            fetch(cur, tile);
+        }
+        if constexpr (STAGE) {
+            // the bulk stores of the previous tile have finished reading the stage (bulk groups belong to thread 0)
+            if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+            __syncthreads();
+            split_compute<L, KIND, TP1, FULL, E, true>(f, cur, TileDst<L, true>{stage, MPYC_TILE_LIMBS}, m, smem, o);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // make the stage visible to the async proxy
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                for (int i = 0; i < m; i++)
+                    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(
+                                     shares + (size_t)i * sstride + tile * MPYC_TILE_LIMBS),
+                                 "r"(smem_u32(stage + (size_t)i * MPYC_TILE_LIMBS)), "n"(MPYC_TILE_LIMBS * 8)
+                                 : "memory");
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        } else {
+            split_compute<L, KIND, TP1, FULL, E, true>(f, cur, TileDst<L, false>{shares, sstride}, m, smem,
+                                                       tile * MPYC_TILE_LIMBS + o);
+        }
+        if (more) {
+#pragma unroll
+            for (int j = 0; j < TP1; j++)
+#pragma unroll
+                for (int q = 0; q < E * N; q++) cur[j][q] = nxt[j][q];
+        }
     }
+    if constexpr (STAGE) {
+        if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // before the stage goes away
+    }
+    // partial last tile: one element per thread, stored directly
+    const size_t nth = (size_t)gridDim.x * blockDim.x;
+    for (size_t h = ntiles * TE + (size_t)blockIdx.x * blockDim.x + threadIdx.x; h < n; h += nth)
+        split_items<L, KIND, TP1, FULL, 1, false, 1>(f, secrets, coeffs, cstride, StridedDst{shares, sstride}, m, smem,
+                                                     h * (size_t)L, 0);
 }
 
 // ---- generate mode: coefficients come from a ChaCha20 keystream and never touch memory ----------

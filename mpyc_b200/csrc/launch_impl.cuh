@@ -131,17 +131,44 @@ static inline FieldParams split_q32(const FieldParams& fp, bool full, int t, int
     return f;
 }
 
+#ifndef MPYC_SPLIT_STAGE_MAX
+// the tiled K2 writes through a shared-memory stage while two CTAs per SM still fit (228 KB of shared memory per SM,
+// 1 KB of it reserved per CTA); larger m store straight from registers (-DMPYC_SPLIT_STAGE_MAX=0: always; experiments)
+#define MPYC_SPLIT_STAGE_MAX (113u * 1024u)
+#endif
+
+template <int L, int KIND, int TP1, bool FULL>
+static cudaError_t split_tiled_k(const FieldParams& fp, const u64* secrets, const u64* coeffs, size_t cstride,
+                                 u64* shares, size_t sstride, size_t n, int m, const u64* gtab, u32 tab_bytes,
+                                 cudaStream_t st) {
+    const size_t ntiles = n / (MPYC_TILE_LIMBS / L);
+    const size_t items = std::max<size_t>(ntiles, 1) * MPYC_THREADS;
+    const size_t smem = ((tab_bytes + 127u) & ~127u) + (size_t)m * MPYC_TILE_LIMBS * sizeof(u64);
+    if (smem <= MPYC_SPLIT_STAGE_MAX) {
+        auto kernel = k_split_tiled<L, KIND, TP1, FULL, true>;
+        if (smem > 48u * 1024u) {
+            cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return e;
+        }
+        return launch_kernel(kernel, items, smem, st, fp, secrets, coeffs, cstride, shares, sstride, n, m, gtab, tab_bytes);
+    }
+    return launch_kernel(k_split_tiled<L, KIND, TP1, FULL, false>, items, tab_bytes, st, fp, secrets, coeffs, cstride,
+                         shares, sstride, n, m, gtab, tab_bytes);
+}
+
 template <int L, int KIND, bool FULL, bool VEC>
 static cudaError_t split_k(const FieldParams& fp, const u64* secrets, const u64* coeffs, size_t cstride, u64* shares,
                            size_t sstride, size_t n, int t, int m, const u64* gtab, u32 tab_bytes, cudaStream_t st) {
-    constexpr int E = VEC ? VecItem<L>::E : 1;
-    size_t items = (n + E - 1) / E;
     constexpr int MAXT = FULL ? 5 : 9;
 #define SPLIT_CASE(T)                                                                                            \
     case T:                                                                                                      \
-        if constexpr (T <= MAXT)                                                                                 \
-            return launch_kernel(k_split<L, KIND, T, FULL, VEC>, items, tab_bytes, st, fp, secrets, coeffs,      \
-                                 cstride, shares, sstride, n, m, gtab, tab_bytes);                               \
+        if constexpr (T <= MAXT) {                                                                               \
+            if constexpr (VEC)                                                                                   \
+                return split_tiled_k<L, KIND, T, FULL>(fp, secrets, coeffs, cstride, shares, sstride, n, m, gtab, \
+                                                       tab_bytes, st);                                           \
+            return launch_kernel(k_split<L, KIND, T, FULL>, n, tab_bytes, st, fp, secrets, coeffs, cstride, shares, \
+                                 sstride, n, m, gtab, tab_bytes);                                                \
+        }                                                                                                        \
         break
     switch (t + 1) {
         SPLIT_CASE(1);
