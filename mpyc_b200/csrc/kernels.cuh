@@ -11,7 +11,8 @@
 //   K2   k_split_tiled (aligned rows; shares leave through shared memory as TMA bulk stores), k_split (small / full
 //        tables; unaligned rows and 3-limb fields), k_split_gen (ChaCha20 coefficients, strided or per-row destinations),
 //        k_split_dyn (any t)                    thresha.py:47-64
-//   K3   k_recombine, k_recombine_small         thresha.py:119-132
+//   K3   k_recombine_tiled (aligned rows; small / full lambda), k_recombine (unaligned rows and 3-limb fields)
+//                                               thresha.py:119-132
 //   K4   k_prss_tiles, k_prss_combine           thresha.py:163-173,201-217
 #pragma once
 #include "ff_arith.cuh"
@@ -311,8 +312,7 @@ k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, in
 //   full : table entry is a full field element in table form; acc (2L+1 limbs), one reduction
 // ---------------------------------------------------------------------------------------
 
-// items in flight per thread (split is fastest without unrolling, recombine with 4 items for 1-limb and 2 items
-// for 2-limb fields); override with -D for experiments
+// items in flight per thread (split is fastest without unrolling); override with -D for experiments
 #ifndef MPYC_SPLIT_U
 #define MPYC_SPLIT_U 1
 #endif
@@ -321,17 +321,8 @@ k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, in
 #ifndef MPYC_SPLIT_MU
 #define MPYC_SPLIT_MU ((L == 1 || KIND == KIND_GENERIC) ? 1 : 2)
 #endif
-#ifndef MPYC_REC_U1
-#define MPYC_REC_U1 2
-#endif
-#ifndef MPYC_REC_U2
-#define MPYC_REC_U2 1
-#endif
-#ifndef MPYC_RECS_U
-#define MPYC_RECS_U 1
-#endif
 
-// Tiled K2 (k_split_tiled): a CTA owns a tile of MPYC_THREADS x 32 bytes of every row (8 KB).  A thread's item is two
+// Tiled K2 and K3 (k_split_tiled, k_recombine_tiled): a CTA owns a tile of MPYC_THREADS x 32 bytes of every row (8 KB).  A thread's item is two
 // 16-byte chunks at tile limb offsets o and o + H: for L <= 2 the chunks tid and tid + MPYC_THREADS, so that a warp
 // load covers 512 contiguous bytes; for L = 4 the two halves of element tid.
 #define MPYC_TILE_LIMBS (MPYC_THREADS * 4)
@@ -522,10 +513,14 @@ k_split_tiled(FieldParams f, const u64* __restrict__ secrets, const u64* __restr
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // make the stage visible to the async proxy
             __syncthreads();
             if (threadIdx.x == 0) {
+                // evict-first: the share rows are not read again by this step, and leaving them in L2 as the most
+                // recent lines slowed the recombination (K3) that follows by up to 10 % (DESIGN.md section 5)
+                u64 pol;
+                asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
                 for (int i = 0; i < m; i++)
-                    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(
+                    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(
                                      shares + (size_t)i * sstride + tile * MPYC_TILE_LIMBS),
-                                 "r"(smem_u32(stage + (size_t)i * MPYC_TILE_LIMBS)), "n"(MPYC_TILE_LIMBS * 8)
+                                 "r"(smem_u32(stage + (size_t)i * MPYC_TILE_LIMBS)), "n"(MPYC_TILE_LIMBS * 8), "l"(pol)
                                  : "memory");
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
@@ -680,157 +675,168 @@ k_split_dyn(FieldParams f, const u64* __restrict__ secrets, const u64* __restric
 }
 
 // ---------------------------------------------------------------------------------------
-// K3: Lagrange recombination.  tab[(r*k + i)*L ..] = lambda[r][i] in table form.
+// K3: Lagrange recombination, out[r] = sum_i lambda[r][i] * row_i for each of the `width` points r.
+//   full : tab[(r*k + i)*L ..] = lambda[r][i] in table form; k full products, lazy sum, one reduction.
+//   small: when every lambda has a signed representative of magnitude < 2^58 -- always the case for
+//          x-coordinates 1..k at 0, where lambda_i = (-1)^(i-1) C(k,i), e.g. the 2t+1 = m shares of a resharing
+//          (runtime.py:672-680) -- the k full-width products become multiplications by 64-bit constants into ONE
+//          (L+1)-limb sum.  tab[2*(r*k+i)] = |lambda|, tab[2*(r*k+i)+1] = sign.
 // ---------------------------------------------------------------------------------------
 
-template <int L, int KIND, int E, bool VEC, int U>
-__device__ __forceinline__ void recombine_items(const FieldParams& f, const RowPtrs& rows, int k, int width,
-                                                const u64* tab, u64* out, size_t ostride, size_t limb_off,
-                                                size_t limb_step) {
-    constexpr int RB = (U * E * L <= 4) ? 4 : 2;   // rows loaded per batch (loads issued before the multiplies)
-    constexpr int N = 2 * L;
+template <int L, int KIND, bool SMALL>
+struct RecSum {
     typedef Fp<L, KIND> F;
+    static constexpr int N = 2 * L;
+    static constexpr int W = SMALL ? F::WSM : F::WACC;   // accumulator words
+    // acc += lambda[idx] * x, idx = r*k + i (warp-uniform)
+    static __device__ __forceinline__ void add(u32* acc, const u32* x, const FieldParams& f, const u64* tab, int idx) {
+        if constexpr (SMALL) {
+            const u64 mag = tab[2 * idx];
+            const bool minus = tab[2 * idx + 1] != 0;
+            // -|lambda| * share = |lambda| * (p - share): one accumulator, one reduction
+            // (p - 0 = p is a fine representative of 0: the sum stays below k 2^58 p)
+            u32 y[N];
+            if (minus) sub_n<N>(y, as32(f.p), x);
+            else copy_n<N>(y, x);
+            F::mac_const(acc, y, mag);
+        } else {
+            u32 lam[N];
+            copy_n<N>(lam, as32(tab + (size_t)idx * L));
+            F::mac(acc, x, lam);
+        }
+    }
+    static __device__ __forceinline__ void reduce(u32* r, u32* acc, const FieldParams& f) {
+        if constexpr (SMALL) F::reduce_small_q32(r, acc, f);
+        else F::finish(r, acc, f);
+    }
+};
+
+// one element (limb offset limb_off in every row) for every point; rows loaded RB at a time, the loads of a batch
+// issued before its multiplies
+template <int L, int KIND, bool SMALL>
+__device__ __forceinline__ void recombine_element(const FieldParams& f, const RowPtrs& rows, int k, int width,
+                                                  const u64* tab, u64* out, size_t ostride, size_t limb_off) {
+    typedef RecSum<L, KIND, SMALL> S;
+    constexpr int RB = 4;
     for (int r = 0; r < width; r++) {
-        u32 acc[U][E][F::WACC];
-#pragma unroll
-        for (int u = 0; u < U; u++)
-#pragma unroll
-            for (int e = 0; e < E; e++) zero_n<F::WACC>(acc[u][e]);
+        u32 acc[S::W];
+        zero_n<S::W>(acc);
         for (int i0 = 0; i0 < k; i0 += RB) {
-            u32 x[RB][U][E * N];
+            u32 x[RB][2 * L];
 #pragma unroll
             for (int b = 0; b < RB; b++)
-                if (i0 + b < k) {
-#pragma unroll
-                    for (int u = 0; u < U; u++)
-                        load_limbs<E * L, VEC>(x[b][u], rows.p[i0 + b] + limb_off + u * limb_step);
-                }
+                if (i0 + b < k) load_limbs<L, false>(x[b], rows.p[i0 + b] + limb_off);
 #pragma unroll
             for (int b = 0; b < RB; b++)
-                if (i0 + b < k) {
-                    u32 lam[N];
-                    copy_n<N>(lam, as32(tab + (size_t)(r * k + i0 + b) * L));
-#pragma unroll
-                    for (int u = 0; u < U; u++)
-#pragma unroll
-                        for (int e = 0; e < E; e++) F::mac(acc[u][e], x[b][u] + e * N, lam);
-                }
+                if (i0 + b < k) S::add(acc, x[b], f, tab, r * k + i0 + b);
         }
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-            u32 res[E * N];
-#pragma unroll
-            for (int e = 0; e < E; e++) F::finish(res + e * N, acc[u][e], f);
-            store_limbs<E * L, VEC>(out + (size_t)r * ostride + limb_off + u * limb_step, res);
-        }
+        u32 res[2 * L];
+        S::reduce(res, acc, f);
+        store_limbs<L, false>(out + (size_t)r * ostride + limb_off, res);
     }
 }
 
-// Small-coefficient form: when every lambda has a signed representative of
-// magnitude < 2^58 -- always the case for x-coordinates 1..k at 0, where lambda_i = (-1)^(i-1) C(k,i),
-// e.g. the 2t+1 = m shares of a resharing (runtime.py:672-680) -- the k full-width products become
-// multiplications by 64-bit constants.  tab[2*(r*k+i)] = |lambda|, tab[2*(r*k+i)+1] = sign.
-template <int L, int KIND, int E, bool VEC, int U>
-__device__ __forceinline__ void recombine_items_small(const FieldParams& f, const RowPtrs& rows, int k, int width,
-                                                      const u64* tab, u64* out, size_t ostride, size_t limb_off,
-                                                      size_t limb_step) {
-    constexpr int RB = (U * E * L <= 4) ? 4 : 2;
-    constexpr int N = 2 * L;
-    typedef Fp<L, KIND> F;
-    for (int r = 0; r < width; r++) {
-        u32 acc[U][E][F::WSM];
-#pragma unroll
-        for (int u = 0; u < U; u++)
-#pragma unroll
-            for (int e = 0; e < E; e++) zero_n<F::WSM>(acc[u][e]);
-        for (int i0 = 0; i0 < k; i0 += RB) {
-            u32 x[RB][U][E * N];
-#pragma unroll
-            for (int b = 0; b < RB; b++)
-                if (i0 + b < k) {
-#pragma unroll
-                    for (int u = 0; u < U; u++)
-                        load_limbs<E * L, VEC>(x[b][u], rows.p[i0 + b] + limb_off + u * limb_step);
-                }
-#pragma unroll
-            for (int b = 0; b < RB; b++)
-                if (i0 + b < k) {
-                    const u64 mag = tab[2 * (r * k + i0 + b)];
-                    const bool minus = tab[2 * (r * k + i0 + b) + 1] != 0;   // warp-uniform
-#pragma unroll
-                    for (int u = 0; u < U; u++)
-#pragma unroll
-                        for (int e = 0; e < E; e++) {
-                            // -|lambda| * share = |lambda| * (p - share): one accumulator, one reduction
-                            // (p - 0 = p is a fine representative of 0: the sum stays below k 2^58 p)
-                            u32 y[N];
-                            if (minus) sub_n<N>(y, as32(f.p), x[b][u] + e * N);
-                            else copy_n<N>(y, x[b][u] + e * N);
-                            F::mac_const(acc[u][e], y, mag);
-                        }
-                }
-        }
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-            u32 res[E * N];
-#pragma unroll
-            for (int e = 0; e < E; e++) F::reduce_small_q32(res + e * N, acc[u][e], f);
-            store_limbs<E * L, VEC>(out + (size_t)r * ostride + limb_off + u * limb_step, res);
-        }
-    }
-}
-
-#ifndef MPYC_RECS_MINB1
-// min resident CTAs per SM for the small-lambda recombination of 1-limb fields: 4 (64 registers) instead of the 2
-// its 88 registers allow (3 % faster on an H100 SXM, DESIGN.md section 5)
-#define MPYC_RECS_MINB1 4
-#endif
-template <int L, int KIND, bool VEC>
-__global__ void __launch_bounds__(MPYC_THREADS, L == 1 ? MPYC_RECS_MINB1 : 1)
-k_recombine_small(FieldParams f, RowPtrs rows, int k, int width, const u64* __restrict__ gtab, u32 tab_bytes,
-                  u64* __restrict__ out, size_t ostride, size_t n) {
-    extern __shared__ __align__(16) u64 stab[];
-    __shared__ __align__(8) u64 mbar;
-    tma_stage_table(stab, gtab, tab_bytes, &mbar);
-    constexpr int E = VEC ? VecItem<L>::E : 1;
-    constexpr int U = (L <= 2) ? MPYC_RECS_U : 1;
-    const size_t nth = (size_t)gridDim.x * blockDim.x;
-    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t n_items = n / E;
-    size_t it = tid;
-    for (; it + (U - 1) * nth < n_items; it += U * nth)
-        recombine_items_small<L, KIND, E, VEC, U>(f, rows, k, width, stab, out, ostride, it * (size_t)(E * L),
-                                                  nth * (size_t)(E * L));
-    for (; it < n_items; it += nth)
-        recombine_items_small<L, KIND, E, VEC, 1>(f, rows, k, width, stab, out, ostride, it * (size_t)(E * L), 0);
-    if constexpr (E > 1) {
-        for (size_t h = n_items * E + tid; h < n; h += nth)
-            recombine_items_small<L, KIND, 1, false, 1>(f, rows, k, width, stab, out, ostride, h * (size_t)L, 0);
-    }
-}
-
-template <int L, int KIND, bool VEC>
+// K3 for rows that are not all 32-byte aligned, and for 3-limb fields: one element per thread and trip
+template <int L, int KIND, bool SMALL>
 __global__ void MPYC_LB
 k_recombine(FieldParams f, RowPtrs rows, int k, int width, const u64* __restrict__ gtab, u32 tab_bytes,
             u64* __restrict__ out, size_t ostride, size_t n) {
     extern __shared__ __align__(16) u64 stab[];
     __shared__ __align__(8) u64 mbar;
     tma_stage_table(stab, gtab, tab_bytes, &mbar);
-    constexpr int E = VEC ? VecItem<L>::E : 1;
-    constexpr int U = (L == 1) ? MPYC_REC_U1 : (L == 2 ? MPYC_REC_U2 : 1);
     const size_t nth = (size_t)gridDim.x * blockDim.x;
-    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t n_items = n / E;
-    size_t it = tid;
-    for (; it + (U - 1) * nth < n_items; it += U * nth)
-        recombine_items<L, KIND, E, VEC, U>(f, rows, k, width, stab, out, ostride, it * (size_t)(E * L),
-                                            nth * (size_t)(E * L));
-    for (; it < n_items; it += nth)
-        recombine_items<L, KIND, E, VEC, 1>(f, rows, k, width, stab, out, ostride, it * (size_t)(E * L), 0);
-    if constexpr (E > 1) {
-        for (size_t h = n_items * E + tid; h < n; h += nth)
-            recombine_items<L, KIND, 1, false, 1>(f, rows, k, width, stab, out, ostride, h * (size_t)L, 0);
+    for (size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x; h < n; h += nth)
+        recombine_element<L, KIND, SMALL>(f, rows, k, width, stab, out, ostride, h * (size_t)L);
+}
+
+// K3 for 32-byte aligned rows of 1-, 2- and 4-limb fields, in K2's tile layout (TileItem): a CTA owns 8 KB of each of
+// the k input rows and of each output row per trip, so that a warp load (and for L <= 2 a warp store) covers 512
+// contiguous bytes.  A 32-byte item per thread, as K3 had before, uses half of every sector a warp access touches.
+// KB > 0 (k <= KB): the thread's chunks of all k rows stay in registers while every point is computed, so each row is
+// read once per tile whatever the width, and the next tile's chunks are requested before the current tile is
+// computed.  KB = 0 (any k): rows are streamed RB at a time for each point, no prefetch.
+// L = 4: a thread's item is one 32-byte element, so its accesses are the half-sector pattern again.  The loads are 7/8
+// of C5's K3 traffic, and the card moves that mix at 98 % of the coalesced rate in that form (stream probe, DESIGN.md
+// section 5).  Results stored through a shared-memory stage with TMA bulk stores measured slower (C5 K3 1.73 vs
+// 1.71 ms), so they are stored from registers.
+template <int L, int KIND, bool SMALL, int KB>
+__global__ void MPYC_LB
+k_recombine_tiled(FieldParams f, RowPtrs rows, int k, int width, const u64* __restrict__ gtab, u32 tab_bytes,
+                  u64* __restrict__ out, size_t ostride, size_t n) {
+    extern __shared__ __align__(16) u64 stab[];
+    __shared__ __align__(8) u64 mbar;
+    tma_stage_table(stab, gtab, tab_bytes, &mbar);
+    typedef RecSum<L, KIND, SMALL> S;
+    constexpr int E = VecItem<L>::E, N = 2 * L;
+    constexpr int TE = MPYC_TILE_LIMBS / L;   // elements per tile
+    constexpr int RB = 4;                      // KB = 0: rows per load batch
+    constexpr int KR = KB > 0 ? KB : 1;
+    const size_t ntiles = n / TE;
+    const u32 o = threadIdx.x * TileItem<L>::STEP;
+    u32 cur[KR][E * N], nxt[KR][E * N];
+    auto fetch = [&](u32 (*X)[E * N], size_t tile) {
+        const size_t off = tile * MPYC_TILE_LIMBS + o;
+#pragma unroll
+        for (int i = 0; i < KR; i++)
+            if (i < k) load_tile_item<L>(X[i], rows.p[i] + off);
+    };
+    // point r of the thread's item (E elements) of this tile
+    auto point = [&](u32* res, int r, size_t tile) {
+        u32 acc[E][S::W];
+#pragma unroll
+        for (int e = 0; e < E; e++) zero_n<S::W>(acc[e]);
+        if constexpr (KB > 0) {
+#pragma unroll
+            for (int i = 0; i < KB; i++)
+                if (i < k) {
+#pragma unroll
+                    for (int e = 0; e < E; e++) S::add(acc[e], cur[i] + e * N, f, stab, r * k + i);
+                }
+        } else {
+            const size_t off = tile * MPYC_TILE_LIMBS + o;
+            for (int i0 = 0; i0 < k; i0 += RB) {
+                u32 x[RB][E * N];
+#pragma unroll
+                for (int b = 0; b < RB; b++)
+                    if (i0 + b < k) load_tile_item<L>(x[b], rows.p[i0 + b] + off);
+#pragma unroll
+                for (int b = 0; b < RB; b++)
+                    if (i0 + b < k) {
+#pragma unroll
+                        for (int e = 0; e < E; e++) S::add(acc[e], x[b] + e * N, f, stab, r * k + i0 + b);
+                    }
+            }
+        }
+#pragma unroll
+        for (int e = 0; e < E; e++) S::reduce(res + e * N, acc[e], f);
+    };
+    size_t tile = blockIdx.x;
+    if constexpr (KB > 0) {
+        if (tile < ntiles) fetch(cur, tile);
     }
+    for (; tile < ntiles; tile += gridDim.x) {
+        const bool more = KB > 0 && tile + gridDim.x < ntiles;
+        if constexpr (KB > 0) {
+            if (more) fetch(nxt, tile + gridDim.x);
+        }
+        for (int r = 0; r < width; r++) {
+            u32 res[E * N];
+            point(res, r, tile);
+            u64* p = out + (size_t)r * ostride + tile * MPYC_TILE_LIMBS + o;
+            stg_v4(p, res);
+            stg_v4(p + TileItem<L>::H, res + 4);
+        }
+        if (more) {
+#pragma unroll
+            for (int i = 0; i < KR; i++)
+#pragma unroll
+                for (int q = 0; q < E * N; q++) cur[i][q] = nxt[i][q];
+        }
+    }
+    // partial last tile: one element per thread, stored directly
+    const size_t nth = (size_t)gridDim.x * blockDim.x;
+    for (size_t h = ntiles * TE + (size_t)blockIdx.x * blockDim.x + threadIdx.x; h < n; h += nth)
+        recombine_element<L, KIND, SMALL>(f, rows, k, width, stab, out, ostride, h * (size_t)L);
 }
 
 // ---------------------------------------------------------------------------------------

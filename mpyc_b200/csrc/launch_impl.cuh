@@ -290,38 +290,50 @@ cudaError_t Launch<L>::split_gen(const FieldParams& fp0, bool full, const ChaCha
 
 // ---- recombine ------------------------------------------------------------------------------
 
+template <int L, int KIND, bool SMALL, int KB>
+static cudaError_t recombine_tiled_k(const FieldParams& fp, const RowPtrs& rows, int k, int width, const u64* gtab,
+                                     u32 tab_bytes, u64* out, size_t ostride, size_t n, cudaStream_t st) {
+    const size_t ntiles = n / (MPYC_TILE_LIMBS / L);
+    return launch_kernel(k_recombine_tiled<L, KIND, SMALL, KB>, std::max<size_t>(ntiles, 1) * MPYC_THREADS, tab_bytes,
+                         st, fp, rows, k, width, gtab, tab_bytes, out, ostride, n);
+}
+
+// The rows stay in registers (and the next tile's are prefetched) while that leaves room for two CTAs per SM: k <= 4
+// for L <= 2 (106-128 registers at k = 3, 4), k <= 2 for L = 4 (74).  Larger k stream their rows: k = 8 in registers
+// takes 166-192 registers, one CTA per SM, and C5's K3 (L = 4, k = 7) 2.19 ms instead of 1.82.
+template <int L, int KIND, bool SMALL>
+static cudaError_t recombine_tiled(const FieldParams& fp, const RowPtrs& rows, int k, int width, const u64* gtab,
+                                   u32 tab_bytes, u64* out, size_t ostride, size_t n, cudaStream_t st) {
+#define GO(KB) return recombine_tiled_k<L, KIND, SMALL, KB>(fp, rows, k, width, gtab, tab_bytes, out, ostride, n, st)
+    if (k <= 2) GO(2);
+    if constexpr (L <= 2) {
+        if (k == 3) GO(3);
+        if (k == 4) GO(4);
+    }
+    GO(0);
+#undef GO
+}
+
 template <int L>
 cudaError_t Launch<L>::recombine(const FieldParams& fp, bool small, const RowPtrs& rows, int k, int width,
                                  const u64* gtab, u32 tab_bytes, u64* out, size_t ostride, size_t n, cudaStream_t st) {
-    bool vec = L != 3 && aligned32(out) && (ostride % 4 == 0 || width <= 1);   // stride in limbs
-    for (int i = 0; i < k; i++) vec = vec && aligned32(rows.p[i]);
-    constexpr int EV = VecItem<L>::E;
-    if (small) {
-#define SM(VECF, ITEMS)                                                                                                  \
-    do {                                                                                                                 \
-        if (fp.kind == KIND_PM_ALIGNED)                                                                                  \
-            return launch_kernel(k_recombine_small<L, KIND_PM_ALIGNED, VECF>, ITEMS, tab_bytes, st, fp, rows, k, width,  \
-                                 gtab, tab_bytes, out, ostride, n);                                                      \
-        if (fp.kind == KIND_PM_SHIFT)                                                                                    \
-            return launch_kernel(k_recombine_small<L, KIND_PM_SHIFT, VECF>, ITEMS, tab_bytes, st, fp, rows, k, width,    \
-                                 gtab, tab_bytes, out, ostride, n);                                                      \
-        return launch_kernel(k_recombine_small<L, KIND_GENERIC, VECF>, ITEMS, tab_bytes, st, fp, rows, k, width, gtab,   \
-                             tab_bytes, out, ostride, n);                                                                \
-    } while (0)
-        if constexpr (L != 3) {
-            if (vec) SM(true, (n + EV - 1) / EV);
-        }
-        SM(false, n);
-#undef SM
-    }
+    if (n == 0) return cudaSuccess;
+    bool tiled = L != 3 && aligned32(out) && (ostride % 4 == 0 || width <= 1);   // stride in limbs
+    for (int i = 0; i < k; i++) tiled = tiled && aligned32(rows.p[i]);
     if constexpr (L != 3) {
-        if (vec) {
-#define M(K) return launch_kernel(k_recombine<L, K, true>, (n + EV - 1) / EV, tab_bytes, st, fp, rows, k, width, gtab, tab_bytes, out, ostride, n)
+        if (tiled) {
+#define M(K)                                                                                                       \
+    return small ? recombine_tiled<L, K, true>(fp, rows, k, width, gtab, tab_bytes, out, ostride, n, st)           \
+                 : recombine_tiled<L, K, false>(fp, rows, k, width, gtab, tab_bytes, out, ostride, n, st)
             KIND_SWITCH(fp.kind, M)
 #undef M
         }
     }
-#define M(K) return launch_kernel(k_recombine<L, K, false>, n, tab_bytes, st, fp, rows, k, width, gtab, tab_bytes, out, ostride, n)
+#define M(K)                                                                                                           \
+    return small ? launch_kernel(k_recombine<L, K, true>, n, tab_bytes, st, fp, rows, k, width, gtab, tab_bytes, out,  \
+                                 ostride, n)                                                                           \
+                 : launch_kernel(k_recombine<L, K, false>, n, tab_bytes, st, fp, rows, k, width, gtab, tab_bytes, out, \
+                                 ostride, n)
     KIND_SWITCH(fp.kind, M)
 #undef M
     return cudaErrorInvalidValue;

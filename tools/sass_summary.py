@@ -14,8 +14,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ = os.path.join(ROOT, 'mpyc_b200', 'csrc', '_obj')
 DEFAULT = [r'k_split_tiled<2, 1, 3, 0, 1>', r'k_split_tiled<2, 0, 3, 0, 1>', r'k_split_tiled<1, 1, 2, 0, 1>', r'k_split_tiled<4, 1, 4, 0, 1>',
-           r'k_split_gen<2, 1, 3, 0, 1, StridedDst>', r'k_recombine_small<2, 1, 1>', r'k_recombine<2, 0, 1>', r'k_recombine<1, 1, 1>',
-           r'k_recombine_small<4, 1, 1>', r'k_binop<1, 1, 2, 0, 1>', r'k_binop<1, 0, 2, 0, 1>', r'k_prss_tiles<4, 1, 1, 1, 1>',
+           r'k_split_gen<2, 1, 3, 0, 1, StridedDst>', r'k_recombine_tiled<2, 1, 1, 3>', r'k_recombine_tiled<2, 0, 1, 3>',
+           r'k_recombine_tiled<1, 1, 1, 2>', r'k_recombine_tiled<4, 1, 1, 8>', r'k_recombine_tiled<2, 0, 0, 4>', r'k_binop<1, 1, 2, 0, 1>', r'k_binop<1, 0, 2, 0, 1>', r'k_prss_tiles<4, 1, 1, 1, 1>',
            r'k_prss_tiles<4, 1, 1, 1, 0>', r'k_matmul<2, 1', r'k_inv_batch<2, 1>', r'k_prf_reduce<', r'k_gf_split', r'k_gf_recombine',
            # K6, the protocols' raw-value algebra (local.cuh): LDGSTS = cp.async pieces of k_bits_compose
            r'k_bits_compose<2, 1>', r'k_bits_compose<1, 1>', r'k_bits_compose<4, 1>', r'k_bits_decompose<2, 1>', r'k_fma<2, 1, 1, 1>',
