@@ -145,6 +145,21 @@ int mpyc_b200_ff_transpose(const mpyc_b200_field* f, const void* d_in, size_t ro
 int mpyc_b200_ff_cumsum_rows(const mpyc_b200_field* f, const void* d_in, size_t rows, size_t cols, void* d_out, void* stream);
 int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                             size_t rows, size_t cols, void* stream);
+/* ---- sums along an axis (K7; prime fields) ----------------------------------------------------
+ * d_in is a C-ordered array viewed as (outer, len, inner): len is the length of the axis, outer the product of the axes
+ * before it, inner the product of the axes after it.  Any 8-byte aligned d_in works (a slice may start at any element).
+ *
+ * np.sum(a, axis, initial=...) / FiniteFieldArray.sum (mpyc/finfields.py:1332-1337, 766-819; Runtime.np_sum,
+ * runtime.py:3476-3506): out[o][i] = (initial + sum_r in[o][r][i]) mod p, out (outer, inner).  initial: L canonical host
+ * limbs, or NULL for 0.  len == 0 writes initial. */
+int mpyc_b200_ff_sum_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                          const uint64_t* initial, void* d_out, void* stream);
+/* np.cumsum(a, axis) / np.cumulative_sum(a, axis, include_initial) (Runtime.np_cumsum / np_cumulative_sum,
+ * runtime.py:3510-3549): out[o][inc + r][i] = sum_{r' <= r} in[o][r'][i] mod p, out (outer, len + inc, inner) with
+ * inc = include_initial != 0 and a zero row first when inc.  d_in and d_out must not overlap. */
+int mpyc_b200_ff_cumsum_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                             int include_initial, void* d_out, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -64,6 +64,8 @@ _SIGNATURES = {
     'mpyc_b200_ff_bits_decompose': (c_int, [_field_p, c_void_p, c_size_t, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     'mpyc_b200_ff_transpose': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     'mpyc_b200_ff_cumsum_rows': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    'mpyc_b200_ff_sum_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, POINTER(c_uint64), c_void_p, c_void_p]),
+    'mpyc_b200_ff_cumsum_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p]),
     'mpyc_b200_ff_binop_rows': (c_int, [_field_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p]),
     'mpyc_b200_ff_conv2d': (c_int, [_field_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),

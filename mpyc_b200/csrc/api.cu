@@ -719,7 +719,48 @@ MPYC_API int mpyc_b200_ff_cumsum_rows(const mpyc_b200_field* f, const void* d_in
     cudaStream_t st = (cudaStream_t)stream;
     return with_limbs((int)f->fp.L, [&](auto Lc) {
         constexpr int L = decltype(Lc)::value;
-        return launch_status(Launch<L>::cumsum_rows(f->fp, (const u64*)d_in, (u64*)d_out, rows, cols, st), "ff_cumsum_rows launch");
+        return launch_status(Launch<L>::scan_axis(f->fp, (const u64*)d_in, (u64*)d_out, 1, rows, cols, false, st), "ff_cumsum_rows launch");
+    });
+}
+
+// ---------------------------------------------------------------------------------------
+// K7: sums and running sums along an axis (reduce.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+// outer * rows * inner elements of L limbs, addressable in bytes
+static bool axis_size_ok(const mpyc_b200_field* f, size_t outer, size_t rows, size_t inner) {
+    size_t n = 0;
+    return !__builtin_mul_overflow(outer, rows, &n) && !__builtin_mul_overflow(n, inner, &n) &&
+           !__builtin_mul_overflow(n, (size_t)f->fp.L * sizeof(u64), &n);
+}
+
+MPYC_API int mpyc_b200_ff_sum_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                                   const uint64_t* initial, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_sum_axis: field is null")) return rc;
+    if (!axis_size_ok(f, outer, len, inner) || !axis_size_ok(f, outer, 1, inner)) return fail(MPYC_B200_EINVAL, "ff_sum_axis: size overflow");
+    if (outer == 0 || inner == 0) return MPYC_B200_OK;
+    if (!d_out || (len && !d_in)) return fail(MPYC_B200_EINVAL, "ff_sum_axis: null buffer");
+    if (initial && !canonical(f, initial)) return fail(MPYC_B200_EINVAL, "ff_sum_axis: initial must be a canonical residue");
+    cudaStream_t st = (cudaStream_t)stream;
+    return with_limbs((int)f->fp.L, [&](auto Lc) {
+        constexpr int L = decltype(Lc)::value;
+        return launch_status(Launch<L>::sum_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, (const u64*)initial, st),
+                             "ff_sum_axis launch");
+    });
+}
+
+MPYC_API int mpyc_b200_ff_cumsum_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                                      int include_initial, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_cumsum_axis: field is null")) return rc;
+    const size_t inc = include_initial ? 1 : 0;
+    if (len > SIZE_MAX - inc || !axis_size_ok(f, outer, len + inc, inner)) return fail(MPYC_B200_EINVAL, "ff_cumsum_axis: size overflow");
+    if (outer == 0 || inner == 0 || len + inc == 0) return MPYC_B200_OK;
+    if (!d_out || (len && !d_in)) return fail(MPYC_B200_EINVAL, "ff_cumsum_axis: null buffer");
+    cudaStream_t st = (cudaStream_t)stream;
+    return with_limbs((int)f->fp.L, [&](auto Lc) {
+        constexpr int L = decltype(Lc)::value;
+        return launch_status(Launch<L>::scan_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, inc != 0, st),
+                             "ff_cumsum_axis launch");
     });
 }
 

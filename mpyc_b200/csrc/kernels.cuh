@@ -14,6 +14,7 @@
 //   K3   k_recombine_tiled (aligned rows; small / full lambda), k_recombine (unaligned rows and 3-limb fields)
 //                                               thresha.py:119-132
 //   K4   k_prss_tiles, k_prss_combine           thresha.py:163-173,201-217
+//   K7   k_sum_cols / k_sum_rows, k_scan_cols / k_scan_rows (reduce.cuh)   np.sum / np.cumsum along any axis
 #pragma once
 #include "ff_arith.cuh"
 
@@ -1146,7 +1147,7 @@ k_prss_tiles(FieldParams f, const unsigned char* __restrict__ bytes, size_t subs
 
 // Split-k form (ksplit > 1; few output rows, long dot products -- e.g. np_cnnmnist's 1 x 3136 @ 3136 x 1024 layer, which
 // has only 4 column tiles): work item w = (slice s, tile) computes the partial products over k-slice s and writes them,
-// reduced, to C + s*r*c; k_sum_slices adds the slices.  ksplit == 1 writes the result itself.
+// reduced, to C + s*r*c; the sum over the slices is K7's (Launch::matmul).  ksplit == 1 writes the result itself.
 template <int L, int KIND, int TM>
 __global__ void MPYC_LB
 k_matmul(FieldParams f, const u64* __restrict__ A, const u64* __restrict__ B, u64* __restrict__ C, size_t r, size_t k,
@@ -1223,23 +1224,6 @@ k_matmul(FieldParams f, const u64* __restrict__ A, const u64* __restrict__ B, u6
     }
 }
 
-// out[e] = sum over the ksplit slices of part[s][e] (mod p), e < count elements
-template <int L, int KIND>
-__global__ void MPYC_LB
-k_sum_slices(FieldParams f, const u64* __restrict__ part, u64* __restrict__ out, size_t count, size_t ksplit) {
-    constexpr int N = 2 * L;
-    const size_t nth = (size_t)gridDim.x * blockDim.x;
-    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < count; e += nth) {
-        u32 acc[N], x[N];
-        load_limbs<L, false>(acc, part + e * L);
-        for (size_t s = 1; s < ksplit; s++) {
-            load_limbs<L, false>(x, part + (s * count + e) * L);
-            Fp<L, KIND>::add(acc, acc, x, f);
-        }
-        store_limbs<L, false>(out + e * L, acc);
-    }
-}
-
 // ---------------------------------------------------------------------------------------
 // utilities
 // ---------------------------------------------------------------------------------------
@@ -1292,3 +1276,4 @@ k_count_mismatch(const u64* __restrict__ a, const u64* __restrict__ b, size_t n_
 }
 
 #include "local.cuh"
+#include "reduce.cuh"

@@ -62,15 +62,20 @@ struct Launch {
     // out[j*ostride + i] = bit e(j) of c[i]   (ostride in elements)
     static cudaError_t bits_decompose(const FieldParams& fp, const u64* c, u64* out, size_t ostride, size_t n, int l, bool descending,
                                       cudaStream_t st);
-    // out (C, R) = in (R, C) transposed; out (R, C) = running sums of in down the rows; out = a (R, C) (op) b (C) broadcast
-    // over the rows (reflected: b (op) a)
+    // out (C, R) = in (R, C) transposed; out = a (R, C) (op) b (C) broadcast over the rows (reflected: b (op) a)
     static cudaError_t transpose(const FieldParams& fp, const u64* in, u64* out, size_t R, size_t C, cudaStream_t st);
-    static cudaError_t cumsum_rows(const FieldParams& fp, const u64* in, u64* out, size_t R, size_t C, cudaStream_t st);
     static cudaError_t binop_rows(const FieldParams& fp, int op, bool reflected, const u64* a, const u64* b, u64* out, size_t R,
                                   size_t C, cudaStream_t st);
     // Y (k, v, m, n) = 'same' correlation of X (k, r, m, n) with W (v, r, s, s) over the r input channels + B (v); s odd
     static cudaError_t conv2d(const FieldParams& fp, const u64* X, const u64* W, const u64* B, u64* Y, int k, int r, int m, int n,
                               int v, int s, cudaStream_t st);
+    // ---- K7: along the middle axis of a C-ordered (O, R, I) array (reduce.cuh) ----
+    // out (O, I) = init + sum_r in (O, R, I); init: L canonical host limbs, or null for 0
+    static cudaError_t sum_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, const u64* init,
+                                cudaStream_t st);
+    // out (O, R + inc, I) = running sums of in (O, R, I) along R, after a zero row when inc; in and out must not overlap
+    static cudaError_t scan_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool inc,
+                                 cudaStream_t st);
 };
 
 extern template struct Launch<1>;

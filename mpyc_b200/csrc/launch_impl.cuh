@@ -425,7 +425,6 @@ cudaError_t Launch<L>::matmul(const FieldParams& fp, const u64* A, const u64* B,
 #define M(K)                                                                                                              \
     e = tm == 4 ? launch_kernel(k_matmul<L, K, 4>, tiles * ksplit * MPYC_THREADS, 0, st, fp, A, B, dst, r, k, c, kslice, ksplit) \
                 : launch_kernel(k_matmul<L, K, 1>, tiles * ksplit * MPYC_THREADS, 0, st, fp, A, B, dst, r, k, c, kslice, ksplit); \
-    if (e == cudaSuccess && ksplit > 1) e = launch_kernel(k_sum_slices<L, K>, r * c, 0, st, fp, part, C, r * c, ksplit);  \
     break
     switch (fp.kind) {
         case KIND_GENERIC: M(KIND_GENERIC);
@@ -434,6 +433,7 @@ cudaError_t Launch<L>::matmul(const FieldParams& fp, const u64* A, const u64* B,
         default: break;
     }
 #undef M
+    if (e == cudaSuccess && ksplit > 1) e = sum_axis(fp, part, C, 1, ksplit, r * c, nullptr, st);   // the slices' sum
     if (part) cudaFreeAsync(part, st);
     return e;
 }
@@ -569,14 +569,6 @@ cudaError_t Launch<L>::transpose(const FieldParams& fp, const u64* in, u64* out,
     return launch_kernel(k_transpose<L>, tiles * MPYC_THREADS, 0, st, in, out, R, C);
 }
 
-template <int L>
-cudaError_t Launch<L>::cumsum_rows(const FieldParams& fp, const u64* in, u64* out, size_t R, size_t C, cudaStream_t st) {
-    if (L % 2 == 0 && (!aligned16(in) || !aligned16(out))) return cudaErrorMisalignedAddress;
-#define M(K) return launch_kernel(k_cumsum_rows<L, K>, C, 0, st, fp, in, out, R, C)
-    KIND_SWITCH(fp.kind, M)
-#undef M
-    return cudaErrorInvalidValue;
-}
 
 template <int L>
 cudaError_t Launch<L>::binop_rows(const FieldParams& fp, int op, bool reflected, const u64* a, const u64* b, u64* out, size_t R,
@@ -597,4 +589,123 @@ cudaError_t Launch<L>::binop_rows(const FieldParams& fp, int op, bool reflected,
 #undef M
 #undef ROWS_CASE
     return cudaErrorInvalidValue;
+}
+
+// ---- K7: sums and running sums along an axis (reduce.cuh) ---------------------------------------
+
+// Split R into S slices of rs rows when the work items of the shape (columns: O*I threads; rows form: O warps) cannot
+// fill the machine.  Slices keep >= 64 rows (columns) / >= 1024 elements (rows form), so that each item still has
+// enough loads in flight.  The partial sums (S, O, I) are then summed (or scanned) along S by the same launcher.
+struct AxisPlan {
+    size_t S, rs;
+};
+static inline AxisPlan axis_plan(size_t O, size_t R, size_t I) {
+    const bool cols = I >= 32;
+    const size_t sms = (size_t)mpyc_sm_count();
+    const size_t items = cols ? O * I : O;
+    const size_t want = cols ? sms * 1024 : sms * 16;
+    const size_t most = cols ? R / 64 : R * I / 1024;
+    size_t S = items < want ? std::min((want + items - 1) / items, most) : 1;
+    if (S < 2) return AxisPlan{1, R};
+    const size_t rs = (R + S - 1) / S;
+    return AxisPlan{(R + rs - 1) / rs, rs};
+}
+
+template <int L, int KIND, bool VEC>
+static cudaError_t sum_pass(const FieldParams& fp0, const u64* in, u64* out, size_t O, size_t R, size_t I, size_t S, size_t rs,
+                            const ScalarParam& init, int add_init, cudaStream_t st) {
+    FieldParams fp = fp0;
+    fp.q32 = rs <= ((size_t)1 << 31) ? 1u : 0u;          // every lazy sum < rs * p <= 2^(k+31)
+    if (I >= 32) return launch_kernel(k_sum_cols<L, KIND, VEC>, S * O * I, 0, st, fp, in, out, O, R, I, rs, S, init, add_init);
+    return launch_kernel(k_sum_rows<L, KIND, VEC>, S * O * 32, 0, st, fp, in, out, O, R, I, rs, S, init, add_init);
+}
+
+template <int L, int KIND, bool VEC>
+static cudaError_t scan_pass(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, size_t S, size_t rs,
+                             const u64* carry, int inc, cudaStream_t st) {
+    if (I >= 32) return launch_kernel(k_scan_cols<L, KIND, VEC>, S * O * I, 0, st, fp, in, out, O, R, I, rs, S, carry, inc);
+    return launch_kernel(k_scan_rows<L, KIND, VEC>, S * O * 32, 0, st, fp, in, out, O, R, I, rs, S, carry, inc);
+}
+
+// the VEC forms (16-byte accesses) need even L and 16-byte aligned arrays; a DeviceArray slice may start at any element
+template <int L>
+static cudaError_t sum_pass_any(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, size_t S, size_t rs,
+                                const ScalarParam& init, int add_init, cudaStream_t st) {
+    if constexpr (L % 2 == 0) {
+        if (aligned16(in) && aligned16(out)) {
+#define M(K) return sum_pass<L, K, true>(fp, in, out, O, R, I, S, rs, init, add_init, st)
+            KIND_SWITCH(fp.kind, M)
+#undef M
+        }
+    }
+#define M(K) return sum_pass<L, K, false>(fp, in, out, O, R, I, S, rs, init, add_init, st)
+    KIND_SWITCH(fp.kind, M)
+#undef M
+    return cudaErrorInvalidValue;
+}
+
+template <int L>
+static cudaError_t scan_pass_any(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, size_t S, size_t rs,
+                                 const u64* carry, int inc, cudaStream_t st) {
+    if constexpr (L % 2 == 0) {
+        if (aligned16(in) && aligned16(out)) {
+#define M(K) return scan_pass<L, K, true>(fp, in, out, O, R, I, S, rs, carry, inc, st)
+            KIND_SWITCH(fp.kind, M)
+#undef M
+        }
+    }
+#define M(K) return scan_pass<L, K, false>(fp, in, out, O, R, I, S, rs, carry, inc, st)
+    KIND_SWITCH(fp.kind, M)
+#undef M
+    return cudaErrorInvalidValue;
+}
+
+template <int L>
+static cudaError_t sum_axis_impl(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I,
+                                 const ScalarParam& init, int add_init, cudaStream_t st) {
+    if (O * I == 0) return cudaSuccess;
+    const AxisPlan pl = axis_plan(O, R, I);
+    if (pl.S == 1) return sum_pass_any<L>(fp, in, out, O, R, I, 1, R, init, add_init, st);
+    u64* part = nullptr;                                 // (S, O, I) slice sums, stream-ordered scratch
+    cudaError_t e = cudaMallocAsync(&part, pl.S * O * I * L * sizeof(u64), st);
+    if (e != cudaSuccess) return e;
+    e = sum_pass_any<L>(fp, in, part, O, R, I, pl.S, pl.rs, init, 0, st);
+    if (e == cudaSuccess) e = sum_axis_impl<L>(fp, part, out, 1, pl.S, O * I, init, add_init, st);
+    cudaFreeAsync(part, st);
+    return e;
+}
+
+// Reduce-then-scan when R is split: slice sums (S, O, I), their inclusive scan along S, then every slice is scanned
+// again from its carry-in.  No CTA waits on another (three launches in stream order); the input is read twice.
+template <int L>
+static cudaError_t scan_axis_impl(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, int inc,
+                                  cudaStream_t st) {
+    if (O * I == 0) return cudaSuccess;
+    const AxisPlan pl = axis_plan(O, R, I);
+    if (pl.S == 1) return scan_pass_any<L>(fp, in, out, O, R, I, 1, R, nullptr, inc, st);
+    const size_t count = pl.S * O * I;
+    u64* part = nullptr;                                 // slice sums, then their running sums
+    cudaError_t e = cudaMallocAsync(&part, 2 * count * L * sizeof(u64), st);
+    if (e != cudaSuccess) return e;
+    const ScalarParam zero = {};
+    e = sum_pass_any<L>(fp, in, part, O, R, I, pl.S, pl.rs, zero, 0, st);
+    if (e == cudaSuccess) e = scan_axis_impl<L>(fp, part, part + count * L, 1, pl.S, O * I, 0, st);
+    if (e == cudaSuccess) e = scan_pass_any<L>(fp, in, out, O, R, I, pl.S, pl.rs, part + count * L, inc, st);
+    cudaFreeAsync(part, st);
+    return e;
+}
+
+template <int L>
+cudaError_t Launch<L>::sum_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, const u64* init,
+                                cudaStream_t st) {
+    ScalarParam sp = {};
+    if (init)
+        for (int i = 0; i < L; i++) sp.v[i] = init[i];
+    return sum_axis_impl<L>(fp, in, out, O, R, I, sp, init ? 1 : 0, st);
+}
+
+template <int L>
+cudaError_t Launch<L>::scan_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool inc,
+                                 cudaStream_t st) {
+    return scan_axis_impl<L>(fp, in, out, O, R, I, inc ? 1 : 0, st);
 }

@@ -11,8 +11,8 @@
 //   k_bits_decompose (c[i] >> e(j)) & 1        np_sgn / np_to_bits: `np.right_shift.outer(c, shifts).T & 1`  :3660, :4423
 //   k_conv2d         'same' 2-D correlation over input channels + bias, mod p
 //                                              demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops)
-//   k_transpose, k_cumsum_rows, k_binop_rows   np_sgn's (l, n) bit-matrix algebra: `r_bits.T`, `np.cumsum(.., axis=0)`,
-//                                              `s_sign - <matrix>` (row broadcast)                 :3661-3672
+//   k_transpose, k_binop_rows                  np_sgn's (l, n) bit-matrix algebra: `r_bits.T`, `s_sign - <matrix>` (row
+//                                              broadcast); its `np.cumsum(.., axis=0)` is K7's scan  :3661-3672
 //
 // The reference computes these over the integers and reduces when the result enters a field array
 // (`Zp.array(...)`, finfields.py:717-725); reduction is a ring homomorphism, so computing mod p throughout gives the
@@ -557,35 +557,6 @@ k_transpose(const u64* __restrict__ in, u64* __restrict__ out, size_t R, size_t 
                     }
                 }
             }
-        }
-    }
-}
-
-// out[j][i] = sum_{j' <= j} in[j'][i] mod p (np.cumsum(axis=0)): a thread walks its column, rows are coalesced
-template <int L, int KIND>
-__global__ void MPYC_LB
-k_cumsum_rows(FieldParams f, const u64* __restrict__ in, u64* __restrict__ out, size_t R, size_t C) {
-    constexpr int N = 2 * L;
-    const size_t nth = (size_t)gridDim.x * blockDim.x;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < C; i += nth) {
-        u32 acc[N];
-        zero_n<N>(acc);
-        size_t j = 0;
-        for (; j + 4 <= R; j += 4) {                     // four rows requested before the first addition
-            u32 x[4][N];
-#pragma unroll
-            for (int q = 0; q < 4; q++) ldg_elem<L>(x[q], in + ((j + q) * C + i) * L);
-#pragma unroll
-            for (int q = 0; q < 4; q++) {
-                Fp<L, KIND>::add(acc, acc, x[q], f);
-                stg_elem<L>(out + ((j + q) * C + i) * L, acc);
-            }
-        }
-        for (; j < R; j++) {
-            u32 x[N];
-            ldg_elem<L>(x, in + (j * C + i) * L);
-            Fp<L, KIND>::add(acc, acc, x, f);
-            stg_elem<L>(out + (j * C + i) * L, acc);
         }
     }
 }

@@ -435,6 +435,43 @@ def cumsum_rows(a: DeviceArray, rows, cols):
     return out
 
 
+def _check_elements(a: DeviceArray, shape, what):
+    n = 1
+    for s in shape:
+        n *= int(s)
+    if a.n != n:
+        raise ValueError(f'{what}: buffer does not hold the {n} elements of shape {tuple(shape)}')
+    a._check_contiguous()
+
+
+def sum_axis(a: DeviceArray, shape, axis=None, keepdims=False, initial=0):
+    """np.sum(a.reshape(shape), axis=axis, keepdims=keepdims, initial=initial) mod p on the K7 kernels (Runtime.np_sum,
+    mpyc/runtime.py:3476-3506; FiniteFieldArray.sum, mpyc/finfields.py:1332-1337).  axis: None, an int or a tuple, negative
+    axes allowed.  Returns (DeviceArray of the result's elements, result shape); a 0-d result is one element."""
+    from mpyc_b200 import axes
+    _check_elements(a, shape, 'sum_axis')
+    passes, out_shape = axes.sum_plan(shape, axis, keepdims)
+    init = a.ctx.scalar_limbs(int(initial) % a.ctx.order)
+    cur = a
+    for j, (O, R, I) in enumerate(passes):
+        out = DeviceArray.empty(a.ctx, O * I, a.t.device)
+        last = j == len(passes) - 1
+        check(lib.mpyc_b200_ff_sum_axis(a.ctx.handle, cur.ptr, O, R, I, init if last else None, out.ptr, _stream_ptr()))
+        cur = out
+    return cur, out_shape
+
+
+def cumsum_axis(a: DeviceArray, shape, axis=None, include_initial=False):
+    """np.cumsum(a.reshape(shape), axis) (axis=None: flattened) and, with include_initial, np.cumulative_sum(...,
+    include_initial=True) mod p on the K7 kernels (mpyc/runtime.py:3510-3549).  Returns (DeviceArray, result shape)."""
+    from mpyc_b200 import axes
+    _check_elements(a, shape, 'cumsum_axis')
+    (O, R, I), out_shape = axes.scan_plan(shape, axis, include_initial)
+    out = DeviceArray.empty(a.ctx, O * (R + (1 if include_initial else 0)) * I, a.t.device)
+    check(lib.mpyc_b200_ff_cumsum_axis(a.ctx.handle, a.ptr, O, R, I, 1 if include_initial else 0, out.ptr, _stream_ptr()))
+    return out, out_shape
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

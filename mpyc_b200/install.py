@@ -113,19 +113,24 @@ _saved_ops = {}
 
 def _install_operators(finfields_module, min_size):
     """FiniteFieldArray.__init__ and + - * neg @ (mpyc/finfields.py:717-725,1056-1146): limb-backed operands, and plain
-    object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident); everything
+    object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
+    np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays; everything
     else -- scalars with small arrays, broadcasting, uncovered fields -- runs the reference's own method unchanged."""
     from mpyc_b200 import _cabi, resident
     resident.min_size = int(min_size)
     cls = finfields_module.FiniteFieldArray
     names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
-             '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__')
+             '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
+             'sum')
     orig = {name: cls.__dict__[name] for name in names}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
     orig_hash = cls.__hash__          # assigning __eq__ on a class does not touch __hash__, kept explicit for clarity
     value_property = resident.make_value_property(finfields_module)
     slot_set = resident._slot.__set__
+    import numpy as np
+    # np.sum / cumsum / cumulative_sum (K7) and np.outer (K1c), mpyc_b200.resident.array_function
+    reductions = tuple(f for f in (np.sum, np.cumsum, getattr(np, 'cumulative_sum', None), np.outer) if f is not None)
 
     def __init__(self, value, check=True, copy=False):
         lv = resident.as_limb_value(value)
@@ -180,7 +185,16 @@ def _install_operators(finfields_module, min_size):
             r = resident.concatenate(type(self), list(args[0]), kwargs.get('axis', 0))
             if r is not MISS:
                 return r
+        if func in reductions and isinstance(self, cls):
+            r = resident.array_function(self, func, args, kwargs)
+            if r is not MISS:
+                return r
         return orig['__array_function__'](self, func, types, args, kwargs)
+
+    def sum(self, *args, **kwargs):
+        # ndarray.sum(axis=None, dtype=None, out=None, keepdims=False, initial=0, where=True)
+        r = resident.array_function(self, np.sum, (self,) + args, kwargs) if len(args) <= 5 else MISS
+        return orig['sum'](self, *args, **kwargs) if r is MISS else r
 
     def __eq__(self, other):
         r = resident.equals(self, other, False)
@@ -195,6 +209,7 @@ def _install_operators(finfields_module, min_size):
     cls.__hash__ = orig_hash
     cls.__getitem__ = __getitem__
     cls.__array_function__ = __array_function__
+    cls.sum = sum
     cls.__lshift__ = make_shift('__lshift__', False, False)
     cls.__rshift__ = make_shift('__rshift__', True, False)
     cls.__ilshift__ = make_shift('__ilshift__', False, True)

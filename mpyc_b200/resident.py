@@ -35,7 +35,7 @@ replaces `backend` by the oracle to exercise this module's host logic where no G
 """
 import numpy as np
 
-from mpyc_b200 import _cabi, codec
+from mpyc_b200 import _cabi, axes, codec
 from mpyc_b200.field import context_for, context_of_field
 from mpyc_b200.wire import ShareRow, _poly_type
 
@@ -152,6 +152,15 @@ class CudaBackend:
     def binop_rows(self, ctx, op, a, b, rows, cols, reflected):
         dev, _ = self._dev()
         return dev.binop_rows(self.to_store(ctx, a), self.to_store(ctx, b), op, rows, cols, reflected)
+
+    def sum_axis(self, ctx, a, shape, axis, keepdims, initial):
+        """store of the elements of np.sum(a.reshape(shape), axis, keepdims=keepdims, initial=initial) mod p"""
+        dev, _ = self._dev()
+        return dev.sum_axis(self.to_store(ctx, a), shape, axis, keepdims, initial)[0]
+
+    def cumsum_axis(self, ctx, a, shape, axis, include_initial):
+        dev, _ = self._dev()
+        return dev.cumsum_axis(self.to_store(ctx, a), shape, axis, include_initial)[0]
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -1168,6 +1177,120 @@ def matmul(self, other, reflected=False):
         return cls.field(LimbValue(ctx, out, (1,), poly)._materialise()[0])
     shape = (c,) if len(sa) == 1 else ((r,) if len(sb) == 1 else (r, c))
     return _wrap(cls, ctx, out, shape)
+
+
+def _reduction_operand(a):
+    """(cls, ctx, store, shape) of a prime-field array that is limb-backed or an object array of at least min_size
+    elements (the rule of binop); None otherwise.  CudaBackend always has K7; a substituted backend without the sum_axis
+    / cumsum_axis pair (a test stand-in) leaves sums to the reference's code, as before K7 existed."""
+    cls = type(a)
+    ctx = _ctx_of(cls)
+    if ctx is None or ctx.binary or not hasattr(backend, 'cumsum_axis') or not hasattr(backend, 'sum_axis'):
+        return None
+    mine = raw_value(a)
+    if as_limb_value(mine) is None and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
+        return None
+    op = _operand(ctx, cls, a)
+    return None if op is None else (cls, ctx) + op
+
+
+def _plain_int(x):
+    return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+
+
+def sum_(a, axis=None, keepdims=False, initial=0):
+    """np.sum(a, axis, keepdims=keepdims, initial=initial) / a.sum(...) (finfields.py:766-819,1332-1337; Runtime.np_sum,
+    runtime.py:3476-3506) on the K7 kernels: a field element for a 0-d result (finfields.py:818), else a limb-backed
+    array.  _MISS for a non-int initial or keepdims, bad axes (NumPy raises its own error), binary fields and arrays that
+    are neither limb-backed nor large."""
+    if not _plain_int(initial) or not isinstance(keepdims, (bool, np.bool_)):
+        return _MISS
+    try:
+        _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
+    except (TypeError, ValueError):
+        return _MISS
+    op = _reduction_operand(a)
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    out = backend.sum_axis(ctx, store, shape, axis, bool(keepdims), int(initial) % ctx.modulus)
+    if out_shape == ():
+        calls['limb_ops'] += 1
+        return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
+    return _wrap(cls, ctx, out, out_shape)
+
+
+def cumsum(a, axis=None, include_initial=False):
+    """np.cumsum(a, axis) (axis=None: flattened) and np.cumulative_sum(a, axis=axis, include_initial=...) on the K7 scan; a
+    limb-backed array, or _MISS as for sum_."""
+    try:
+        _, out_shape = axes.scan_plan(np.shape(raw_value(a)), axis, include_initial)
+    except (TypeError, ValueError):
+        return _MISS
+    op = _reduction_operand(a)
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    return _wrap(cls, ctx, backend.cumsum_axis(ctx, store, shape, axis, bool(include_initial)), out_shape)
+
+
+def outer(a, b):
+    """np.outer(a, b) of two arrays of one prime field (Runtime.np_outer, runtime.py:2544-2578): c[i, j] = a_i b_j on the
+    flattened operands, through K1c with k = 1.  _MISS for anything else -- a public integer operand in particular, whose
+    values _operand would pack without reducing them."""
+    cls = type(a)
+    ctx = _ctx_of(cls)
+    if ctx is None or ctx.binary or type(b) is not cls:
+        return _MISS
+    va, vb = raw_value(a), raw_value(b)
+    limbish = as_limb_value(va) is not None or as_limb_value(vb) is not None
+    na, nb = int(np.size(va)), int(np.size(vb))
+    if not limbish and na * nb < min_size:
+        return _MISS
+    saved = min_size
+    try:
+        globals()['min_size'] = 0         # both operands are packed whatever their size
+        x = _operand(ctx, cls, a)
+        y = _operand(ctx, cls, b)
+    finally:
+        globals()['min_size'] = saved
+    if x is None or y is None:
+        return _MISS
+    return _wrap(cls, ctx, backend.matmul(ctx, x[0], y[0], na, 1, nb), (na, nb))
+
+
+def array_function(self, func, args, kwargs):
+    """The NumPy functions routed to K7 / K1c by FiniteFieldArray.__array_function__ (install._install_operators):
+    np.sum, np.cumsum, np.cumulative_sum, np.outer.  Arguments are bound as NumPy's signatures do; dtype / out / where
+    and unknown arguments leave the call to the reference (_MISS)."""
+    name = func.__name__
+    if name == 'cumulative_sum':
+        if len(args) != 1 or not set(kwargs) <= {'axis', 'include_initial', 'dtype', 'out'}:
+            return _MISS
+        bound = dict(kwargs, x=args[0])
+        names = ('x',)
+    else:
+        names = {'sum': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'), 'cumsum': ('a', 'axis', 'dtype', 'out'),
+                 'outer': ('a', 'b', 'out')}.get(name)
+        if names is None or len(args) > len(names) or not set(kwargs) <= set(names[len(args):]):
+            return _MISS
+        bound = dict(zip(names, args), **kwargs)
+    if any(bound.get(k, None) is not None for k in ('dtype', 'out')) or bound.get('where', np._NoValue) is not np._NoValue:
+        return _MISS
+    first = bound.get(names[0])
+    if type(first) is not type(self):
+        return _MISS
+    opt = lambda k, default: default if bound.get(k, np._NoValue) is np._NoValue else bound[k]   # noqa: E731
+    if name == 'sum':
+        return sum_(first, opt('axis', None), opt('keepdims', False), opt('initial', 0))
+    if name == 'cumsum':
+        return cumsum(first, opt('axis', None))
+    if name == 'outer':
+        return outer(first, bound.get('b'))
+    axis = opt('axis', None)
+    if axis is None and np.ndim(raw_value(first)) > 1:
+        return _MISS                      # NumPy requires the axis of a multi-dimensional array
+    return cumsum(first, axis, bool(opt('include_initial', False)))
 
 
 def conv2d(x, W, b):

@@ -118,7 +118,7 @@ for step in "$@"; do
       cd $OLDPWD; cat $OUT/r02_demos2.txt ;;
     localncu)
       # one ncu --set full capture per K6 elementwise / matrix kernel (second launch of each), 128-bit field
-      ncu --set full --clock-control none -k regex:"k_fma|k_axpb|k_low_bits|k_nonzero|k_bits_decompose|k_transpose|k_cumsum_rows|k_binop_rows" \
+      ncu --set full --clock-control none -k regex:"k_fma|k_axpb|k_low_bits|k_nonzero|k_bits_decompose|k_transpose|k_scan_cols|k_scan_rows|k_binop_rows" \
           -o $OUT/r02_ncu_local -f python tools/time_local.py --ncu-all > $OUT/r02_ncu_local.log 2>&1
       python tools/ncu_summary.py $OUT/r02_ncu_local.ncu-rep $OUT/r02_ncu_local.txt > /dev/null 2>&1 || true
       rm -f $OUT/r02_ncu_local.ncu-rep

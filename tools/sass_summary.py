@@ -19,7 +19,7 @@ DEFAULT = [r'k_split_tiled<2, 1, 3, 0, 1>', r'k_split_tiled<2, 0, 3, 0, 1>', r'k
            r'k_prss_tiles<4, 1, 1, 1, 0>', r'k_matmul<2, 1', r'k_inv_batch<2, 1>', r'k_prf_reduce<', r'k_gf_split', r'k_gf_recombine',
            # K6, the protocols' raw-value algebra (local.cuh): LDGSTS = cp.async pieces of k_bits_compose
            r'k_bits_compose<2, 1>', r'k_bits_compose<1, 1>', r'k_bits_compose<4, 1>', r'k_bits_decompose<2, 1>', r'k_fma<2, 1, 1, 1>',
-           r'k_axpb<2, 1, 1>', r'k_low_bits<2, 1>', r'k_nonzero<2, 1>', r'k_transpose<2>', r'k_cumsum_rows<2, 1>', r'k_binop_rows<2, 1, 1, 1>',
+           r'k_axpb<2, 1, 1>', r'k_low_bits<2, 1>', r'k_nonzero<2, 1>', r'k_transpose<2>', r'k_scan_cols<2, 1, true>', r'k_binop_rows<2, 1, 1, 1>',
            r'k_conv2d<2, 1>']
 
 
