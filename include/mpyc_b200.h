@@ -160,6 +160,36 @@ int mpyc_b200_ff_sum_axis(const mpyc_b200_field* f, const void* d_in, size_t out
 int mpyc_b200_ff_cumsum_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
                              int include_initial, void* d_out, void* stream);
 
+/* ---- strided views, joins and broadcasts (K8) --------------------------------------------------
+ * A view of a buffer of `len` elements: element (c_0, .., c_{rank-1}) is at
+ *   offset + sum_k o_k * stride[k],  o_k = index[c_k] on index_axis, else c_k
+ * Strides are signed element counts (negative: a flip, 0: a broadcast axis).  index (host memory, extent[index_axis]
+ * int64 entries) is uploaded by the call; index_axis = -1 for none.  Every element of a non-empty view must lie in
+ * [0, len); rank <= MPYC_B200_VIEW_RANK (the caller collapses adjacent axes first). */
+#define MPYC_B200_VIEW_RANK 6
+typedef struct {
+    int64_t offset;
+    int32_t rank;
+    int32_t index_axis;
+    int64_t extent[MPYC_B200_VIEW_RANK];
+    int64_t stride[MPYC_B200_VIEW_RANK];
+    const int64_t* index;
+} mpyc_b200_view;
+/* dst view <- src view, elements of elem_bytes in {1 (GF(2^8)), 8, 16, 24, 32} (any field: layout does not depend on it).
+ * Both views have the same rank and extents; the buffers must not overlap.  Replaces the copies behind NumPy's views of
+ * field arrays: FiniteFieldArray.__getitem__ / __setitem__ (mpyc/finfields.py:1004-1029), transpose / swapaxes / T
+ * (:1358-1368) and np.concatenate / stack / flip / roll / moveaxis through __array_function__ (:766-819); used by
+ * Runtime.np_getitem / np_update / np_transpose / np_concatenate / np_stack / np_flip / np_roll, np_sort, np_argmax and
+ * np_add_bits (mpyc/runtime.py:1758-1773, 2657-2679, 3741-3820, 4310-4325). */
+int mpyc_b200_copy_view(size_t elem_bytes, const void* d_src, size_t src_len, const mpyc_b200_view* src, void* d_dst,
+                        size_t dst_len, const mpyc_b200_view* dst, void* stream);
+/* out = a (op) b mod p on prime fields, op ADD / SUB / MUL: a and b are views (no index axis) whose extents are the
+ * broadcast shape, out is contiguous in C order of it; a broadcast operand is read in place (stride 0).  out must not
+ * overlap a or b.  NumPy's broadcasting of FiniteFieldArray + - * (mpyc/finfields.py:1056-1124), e.g. np_add_bits'
+ * `c1[..., -1, np.newaxis] * d2` (mpyc/runtime.py:4310-4325). */
+int mpyc_b200_ff_binop_view(const mpyc_b200_field* f, int op, const void* d_a, size_t a_len, const mpyc_b200_view* a,
+                            const void* d_b, size_t b_len, const mpyc_b200_view* b, void* d_out, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

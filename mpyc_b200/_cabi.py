@@ -37,7 +37,17 @@ def _load():
 
 lib = _load()
 
+VIEW_RANK = 6
+
+
+class View(ctypes.Structure):
+    """mpyc_b200_view: a strided view of an element buffer (include/mpyc_b200.h)."""
+    _fields_ = [('offset', c_int64), ('rank', ctypes.c_int32), ('index_axis', ctypes.c_int32),
+                ('extent', c_int64 * VIEW_RANK), ('stride', c_int64 * VIEW_RANK), ('index', POINTER(c_int64))]
+
+
 _field_p = c_void_p
+_view_p = POINTER(View)
 _SIGNATURES = {
     'mpyc_b200_version': (c_int, []),
     'mpyc_b200_strerror': (c_char_p, [c_int]),
@@ -66,6 +76,9 @@ _SIGNATURES = {
     'mpyc_b200_ff_cumsum_rows': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     'mpyc_b200_ff_sum_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, POINTER(c_uint64), c_void_p, c_void_p]),
     'mpyc_b200_ff_cumsum_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p]),
+    'mpyc_b200_copy_view': (c_int, [c_size_t, c_void_p, c_size_t, _view_p, c_void_p, c_size_t, _view_p, c_void_p]),
+    'mpyc_b200_ff_binop_view': (c_int, [_field_p, c_int, c_void_p, c_size_t, _view_p, c_void_p, c_size_t, _view_p, c_void_p,
+                                        c_void_p]),
     'mpyc_b200_ff_binop_rows': (c_int, [_field_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p]),
     'mpyc_b200_ff_conv2d': (c_int, [_field_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),

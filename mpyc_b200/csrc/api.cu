@@ -764,6 +764,115 @@ MPYC_API int mpyc_b200_ff_cumsum_axis(const mpyc_b200_field* f, const void* d_in
     });
 }
 
+// ---------------------------------------------------------------------------------------
+// K8: strided views, joins and broadcast arithmetic (layout.cuh)
+// ---------------------------------------------------------------------------------------
+
+// A view's element count (0 if empty) after checking its shape and that every element lies in [0, len): the lowest and
+// highest offsets are offset + the sum over axes of the extreme o_k * stride[k].  Returns -1 on a bad view.
+static long long view_check(const mpyc_b200_view* v, size_t len, bool allow_index) {
+    if (!v || v->rank < 0 || v->rank > MPYC_B200_VIEW_RANK) return -1;
+    if (v->index_axis != -1 && (!allow_index || v->index_axis < 0 || v->index_axis >= v->rank || !v->index)) return -1;
+    long long n = 1;
+    for (int k = 0; k < v->rank; k++) {
+        if (v->extent[k] < 0 || __builtin_mul_overflow(n, v->extent[k], &n)) return -1;
+    }
+    if (n == 0) return 0;
+    __int128 lo = v->offset, hi = v->offset;
+    for (int k = 0; k < v->rank; k++) {
+        int64_t omin = 0, omax = v->extent[k] - 1;
+        if (k == v->index_axis) {
+            omin = omax = v->index[0];
+            for (int64_t c = 1; c < v->extent[k]; c++) omin = std::min(omin, v->index[c]), omax = std::max(omax, v->index[c]);
+        }
+        const __int128 a = (__int128)omin * v->stride[k], b = (__int128)omax * v->stride[k];
+        lo += std::min(a, b);
+        hi += std::max(a, b);
+    }
+    if (lo < 0 || hi >= (__int128)len) return -1;
+    return n;
+}
+
+static bool bytes_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+    return na && nb && x < y + nb && y < x + na;
+}
+
+static bool same_extents(const mpyc_b200_view* a, const mpyc_b200_view* b) {
+    if (a->rank != b->rank) return false;
+    for (int k = 0; k < a->rank; k++)
+        if (a->extent[k] != b->extent[k]) return false;
+    return true;
+}
+
+MPYC_API int mpyc_b200_copy_view(size_t elem_bytes, const void* d_src, size_t src_len, const mpyc_b200_view* src, void* d_dst,
+                                 size_t dst_len, const mpyc_b200_view* dst, void* stream) {
+    if (elem_bytes != 1 && elem_bytes != 8 && elem_bytes != 16 && elem_bytes != 24 && elem_bytes != 32)
+        return fail(MPYC_B200_EINVAL, "copy_view: element size must be 1, 8, 16, 24 or 32 bytes");
+    size_t sb = 0, db = 0;
+    if (__builtin_mul_overflow(src_len, elem_bytes, &sb) || __builtin_mul_overflow(dst_len, elem_bytes, &db))
+        return fail(MPYC_B200_EINVAL, "copy_view: buffer size overflow");
+    const long long ns = view_check(src, src_len, true), nd = view_check(dst, dst_len, true);
+    if (ns < 0 || nd < 0) return fail(MPYC_B200_EINVAL, "copy_view: bad view (rank > 6, negative extent or outside its buffer)");
+    if (!same_extents(src, dst)) return fail(MPYC_B200_EINVAL, "copy_view: views of different extents");
+    if (ns == 0) return MPYC_B200_OK;
+    if (!d_src || !d_dst) return fail(MPYC_B200_EINVAL, "copy_view: null buffer");
+    if (bytes_overlap(d_src, sb, d_dst, db)) return fail(MPYC_B200_EINVAL, "copy_view: source and destination overlap");
+    CopyPlan p = {};
+    p.rank = src->rank;
+    p.six = src->index_axis, p.dix = dst->index_axis;
+    p.soff = src->offset, p.doff = dst->offset;
+    for (int k = 0; k < p.rank; k++) p.ext[k] = src->extent[k], p.sstr[k] = src->stride[k], p.dstr[k] = dst->stride[k];
+    cudaStream_t st = (cudaStream_t)stream;
+    // index tables: uploaded into stream-ordered scratch, freed after the copy
+    const size_t ni = p.six >= 0 ? (size_t)p.ext[p.six] : 0, nj = p.dix >= 0 ? (size_t)p.ext[p.dix] : 0;
+    long long* tab = nullptr;
+    if (ni + nj) {
+        CU(cudaMallocAsync(&tab, (ni + nj) * sizeof(long long), st));
+        cudaError_t e = cudaSuccess;
+        if (ni) e = cudaMemcpyAsync(tab, src->index, ni * sizeof(long long), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess && nj) e = cudaMemcpyAsync(tab + ni, dst->index, nj * sizeof(long long), cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) {
+            cudaFreeAsync(tab, st);
+            return cuda_fail(e, "copy_view: index upload");
+        }
+        p.sidx = ni ? tab : nullptr;
+        p.didx = nj ? tab + ni : nullptr;
+    }
+    const cudaError_t e = launch_copy_view(p, elem_bytes, d_src, d_dst, st);
+    if (tab) cudaFreeAsync(tab, st);
+    return launch_status(e, "copy_view launch");
+}
+
+MPYC_API int mpyc_b200_ff_binop_view(const mpyc_b200_field* f, int op, const void* d_a, size_t a_len, const mpyc_b200_view* a,
+                                     const void* d_b, size_t b_len, const mpyc_b200_view* b, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_binop_view: field is null")) return rc;
+    if (op < 0 || op > 2) return fail(MPYC_B200_EINVAL, "ff_binop_view: op must be ADD, SUB or MUL");
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t ab = 0, bb = 0, ob = 0;
+    if (__builtin_mul_overflow(a_len, E, &ab) || __builtin_mul_overflow(b_len, E, &bb))
+        return fail(MPYC_B200_EINVAL, "ff_binop_view: buffer size overflow");
+    const long long na = view_check(a, a_len, false), nb = view_check(b, b_len, false);
+    if (na < 0 || nb < 0) return fail(MPYC_B200_EINVAL, "ff_binop_view: bad view (rank > 6, negative extent, index table or outside its buffer)");
+    if (!same_extents(a, b)) return fail(MPYC_B200_EINVAL, "ff_binop_view: views of different extents");
+    if (na == 0) return MPYC_B200_OK;
+    if (__builtin_mul_overflow((size_t)na, E, &ob)) return fail(MPYC_B200_EINVAL, "ff_binop_view: size overflow");
+    if (!d_a || !d_b || !d_out) return fail(MPYC_B200_EINVAL, "ff_binop_view: null buffer");
+    if (bytes_overlap(d_out, ob, d_a, ab) || bytes_overlap(d_out, ob, d_b, bb))
+        return fail(MPYC_B200_EINVAL, "ff_binop_view: out overlaps an operand");
+    BinopPlan p = {};
+    p.rank = a->rank;
+    p.aoff = a->offset, p.boff = b->offset;
+    for (int k = 0; k < p.rank; k++) p.ext[k] = a->extent[k], p.astr[k] = a->stride[k], p.bstr[k] = b->stride[k];
+    if (p.rank == 0) p.rank = 1, p.ext[0] = 1;
+    cudaStream_t st = (cudaStream_t)stream;
+    return with_limbs((int)f->fp.L, [&](auto Lc) {
+        constexpr int L = decltype(Lc)::value;
+        return launch_status(Launch<L>::binop_view(f->fp, op, p, (const u64*)d_a, (const u64*)d_b, (u64*)d_out, st),
+                             "ff_binop_view launch");
+    });
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

@@ -15,6 +15,7 @@
 //                                               thresha.py:119-132
 //   K4   k_prss_tiles, k_prss_combine           thresha.py:163-173,201-217
 //   K7   k_sum_cols / k_sum_rows, k_scan_cols / k_scan_rows (reduce.cuh)   np.sum / np.cumsum along any axis
+//   K8   k_copy_gather, k_copy_permute, k_binop_view (layout.cuh)   strided views, joins, broadcast arithmetic
 #pragma once
 #include "ff_arith.cuh"
 
@@ -1277,3 +1278,4 @@ k_count_mismatch(const u64* __restrict__ a, const u64* __restrict__ b, size_t n_
 
 #include "local.cuh"
 #include "reduce.cuh"
+#include "layout.cuh"

@@ -76,7 +76,15 @@ struct Launch {
     // out (O, R + inc, I) = running sums of in (O, R, I) along R, after a zero row when inc; in and out must not overlap
     static cudaError_t scan_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool inc,
                                  cudaStream_t st);
+    // ---- K8: broadcast arithmetic on views (layout.cuh) ----
+    // out (C order over pl.ext) = a_view (op) b_view, op in {OP_ADD, OP_SUB, OP_MUL}
+    static cudaError_t binop_view(const FieldParams& fp, int op, const BinopPlan& pl, const u64* a, const u64* b, u64* out,
+                                  cudaStream_t st);
 };
+
+// K8 (inst_layout.cu): dst_view <- src_view for elements of elem_bytes in {1, 8, 16, 24, 32}; the views are validated and
+// their index tables (if any) are in device memory
+cudaError_t launch_copy_view(const CopyPlan& pl, size_t elem_bytes, const void* src, void* dst, cudaStream_t st);
 
 extern template struct Launch<1>;
 extern template struct Launch<2>;

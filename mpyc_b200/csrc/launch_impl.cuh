@@ -709,3 +709,24 @@ cudaError_t Launch<L>::scan_axis(const FieldParams& fp, const u64* in, u64* out,
                                  cudaStream_t st) {
     return scan_axis_impl<L>(fp, in, out, O, R, I, inc ? 1 : 0, st);
 }
+
+// ---- K8: broadcast arithmetic on views (layout.cuh) ---------------------------------------------
+
+template <int L>
+cudaError_t Launch<L>::binop_view(const FieldParams& fp, int op, const BinopPlan& pl, const u64* a, const u64* b, u64* out,
+                                  cudaStream_t st) {
+    size_t n = 1;
+    for (int k = 0; k < pl.rank; k++) n *= (size_t)pl.ext[k];
+#define VIEW_CASE(K, OPC) return launch_kernel(k_binop_view<L, K, OPC>, n, 0, st, fp, pl, a, b, out, n)
+#define M(K)                                   \
+    switch (op) {                              \
+        case OP_ADD: VIEW_CASE(K, OP_ADD);     \
+        case OP_SUB: VIEW_CASE(K, OP_SUB);     \
+        case OP_MUL: VIEW_CASE(K, OP_MUL);     \
+        default: return cudaErrorInvalidValue; \
+    }
+    KIND_SWITCH(fp.kind, M)
+#undef M
+#undef VIEW_CASE
+    return cudaErrorInvalidValue;
+}

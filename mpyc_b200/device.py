@@ -472,6 +472,49 @@ def cumsum_axis(a: DeviceArray, shape, axis=None, include_initial=False):
     return out, out_shape
 
 
+def _view(v, index_keep):
+    """mpyc_b200.layout.View -> the C struct (its index table stays alive in index_keep)."""
+    c = _cabi.View()
+    c.offset, c.rank, c.index_axis = v.offset, len(v.shape), v.index_axis
+    if c.rank > _cabi.VIEW_RANK:
+        raise ValueError(f'view of rank {c.rank} > {_cabi.VIEW_RANK}: collapse it first (mpyc_b200.layout.collapse)')
+    for k, (e, s) in enumerate(zip(v.shape, v.strides)):
+        c.extent[k], c.stride[k] = e, s
+    if v.index_axis >= 0:
+        idx = np.ascontiguousarray(v.index, dtype=np.int64)
+        index_keep.append(idx)
+        c.index = idx.ctypes.data_as(ctypes.POINTER(ctypes.c_int64))
+    return c
+
+
+def _elem_bytes(ctx):
+    return 1 if ctx.binary else 8 * ctx.nlimbs
+
+
+def copy_view(src: DeviceArray, src_view, dst: DeviceArray, dst_view):
+    """dst[dst_view] <- src[src_view] on the K8 kernels, for views (mpyc_b200.layout.View) of equal extents; any field.
+    Index tables are uploaded from the views' NumPy arrays."""
+    if src.ctx is not dst.ctx:
+        raise ValueError('copy_view: arrays of different fields')
+    keep = []
+    sv, dv = _view(src_view, keep), _view(dst_view, keep)
+    check(lib.mpyc_b200_copy_view(_elem_bytes(src.ctx), src.ptr, src.n, ctypes.byref(sv), dst.ptr, dst.n, ctypes.byref(dv),
+                                  _stream_ptr()))
+
+
+def binop_view(a: DeviceArray, a_view, b: DeviceArray, b_view, op):
+    """a[a_view] (op) b[b_view] into a new contiguous array (C order of the views' extents) on the K8 kernel; op
+    _cabi.OP_ADD / OP_SUB / OP_MUL, prime fields."""
+    if a.ctx is not b.ctx:
+        raise ValueError('binop_view: arrays of different fields')
+    keep = []
+    av, bv = _view(a_view, keep), _view(b_view, keep)
+    out = DeviceArray.empty(a.ctx, a_view.size, a.t.device)
+    check(lib.mpyc_b200_ff_binop_view(a.ctx.handle, op, a.ptr, a.n, ctypes.byref(av), b.ptr, b.n, ctypes.byref(bv), out.ptr,
+                                      _stream_ptr()))
+    return out
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

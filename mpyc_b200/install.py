@@ -114,14 +114,15 @@ _saved_ops = {}
 def _install_operators(finfields_module, min_size):
     """FiniteFieldArray.__init__ and + - * neg @ (mpyc/finfields.py:717-725,1056-1146): limb-backed operands, and plain
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
-    np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays; everything
-    else -- scalars with small arrays, broadcasting, uncovered fields -- runs the reference's own method unchanged."""
+    np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays.  Views, writes,
+    axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout); everything
+    else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
     from mpyc_b200 import _cabi, resident
     resident.min_size = int(min_size)
     cls = finfields_module.FiniteFieldArray
     names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
              '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
-             'sum')
+             'sum', '__setitem__', 'transpose', 'swapaxes')
     orig = {name: cls.__dict__[name] for name in names}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
@@ -179,9 +180,27 @@ def _install_operators(finfields_module, min_size):
         r = resident.getitem(self, key)
         return orig['__getitem__'](self, key) if r is MISS else r
 
+    def __setitem__(self, key, value):
+        if resident.setitem(self, key, value) is MISS:
+            orig['__setitem__'](self, key, value)
+
+    def transpose(self, *axes):
+        # T is self.transpose() (finfields.py:1366-1368)
+        r = resident.permute(self, lambda nd: resident.layout.transpose_axes(nd, axes))
+        return orig['transpose'](self, *axes) if r is MISS else r
+
+    def swapaxes(self, axis1, axis2):
+        r = resident.permute(self, lambda nd: resident.layout.swapaxes_axes(nd, axis1, axis2))
+        return orig['swapaxes'](self, axis1, axis2) if r is MISS else r
+
     def __array_function__(self, func, types, args, kwargs):
         import numpy as np
-        if func is np.concatenate and isinstance(self, cls) and len(args) == 1 and set(kwargs) <= {'axis'}:
+        if func in resident.LAYOUT_FUNCTIONS and isinstance(self, cls):
+            r = resident.layout_function(type(self), func, args, kwargs)
+            if r is not MISS:
+                return r
+        if (func is np.concatenate and isinstance(self, cls) and len(args) == 1 and set(kwargs) <= {'axis'}
+                and not resident._layout_backend()):                   # without K8: axis-0 joins of limb-backed arrays
             r = resident.concatenate(type(self), list(args[0]), kwargs.get('axis', 0))
             if r is not MISS:
                 return r
@@ -208,6 +227,9 @@ def _install_operators(finfields_module, min_size):
     cls.__ne__ = __ne__
     cls.__hash__ = orig_hash
     cls.__getitem__ = __getitem__
+    cls.__setitem__ = __setitem__
+    cls.transpose = transpose
+    cls.swapaxes = swapaxes
     cls.__array_function__ = __array_function__
     cls.sum = sum
     cls.__lshift__ = make_shift('__lshift__', False, False)

@@ -35,7 +35,7 @@ replaces `backend` by the oracle to exercise this module's host logic where no G
 """
 import numpy as np
 
-from mpyc_b200 import _cabi, axes, codec
+from mpyc_b200 import _cabi, axes, codec, layout
 from mpyc_b200.field import context_for, context_of_field
 from mpyc_b200.wire import ShareRow, _poly_type
 
@@ -162,6 +162,23 @@ class CudaBackend:
         dev, _ = self._dev()
         return dev.cumsum_axis(self.to_store(ctx, a), shape, axis, include_initial)[0]
 
+    def copy_view(self, ctx, n, base, items):
+        """A new store of n elements: a copy of the store `base` (None: uninitialised), then dst_view <- src_view for each
+        (src store, src View, dst View) of `items` (K8; views of mpyc_b200.layout)."""
+        dev, where = self._dev()
+        if base is not None:
+            out = dev.DeviceArray(ctx, self.to_store(ctx, base).t.clone())
+        else:
+            out = dev.DeviceArray.empty(ctx, n, where)
+        for st, sv, dv in items:
+            dev.copy_view(self.to_store(ctx, st), sv, out, dv)
+        return out
+
+    def binop_view(self, ctx, op, a, a_view, b, b_view):
+        """store of a[a_view] (op) b[b_view] in C order of the views' (broadcast) extents (K8)"""
+        dev, _ = self._dev()
+        return dev.binop_view(self.to_store(ctx, a), a_view, self.to_store(ctx, b), b_view, op)
+
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
         return dev.conv2d(self.to_store(ctx, X), self.to_store(ctx, W), self.to_store(ctx, B), k, r, m, n, v, s)
@@ -255,7 +272,8 @@ class LimbValue:
         return self.shape[0]
 
     def reshape(self, *shape, **kwargs):
-        if self.store is None or kwargs:
+        # order='C' (Runtime.np_reshape passes it, runtime.py:2746) is the order the limbs are in
+        if self.store is None or (kwargs and kwargs != {'order': 'C'}):
             return self._materialise().reshape(*shape, **kwargs)
         return LimbValue(self.ctx, self.store, _norm_shape(self.size, shape), self._poly)
 
@@ -1033,8 +1051,8 @@ def binop(self, other, op, reflected=False):
     if b is None:
         return _MISS
     if b[1] != a[1]:
-        # NumPy's row broadcast between a matrix (R, C) and a vector (C,) runs on k_binop_rows; any other broadcast stays
-        # with NumPy
+        # NumPy's row broadcast between a matrix (R, C) and a vector (C,) runs on k_binop_rows, any other broadcast on
+        # K8's k_binop_view
         if ctx.binary:
             return _MISS
         if len(a[1]) == 2 and len(b[1]) == 1 and a[1][1] == b[1][0] and a[1][0] and a[1][1]:
@@ -1042,47 +1060,257 @@ def binop(self, other, op, reflected=False):
         elif len(a[1]) == 1 and len(b[1]) == 2 and b[1][1] == a[1][0] and b[1][0] and b[1][1]:
             mat, vec, vec_first = b, a, not reflected
         else:
-            return _MISS
+            return _broadcast_binop(cls, ctx, op, (b, a) if reflected else (a, b))
         R, C = mat[1]
         return _wrap(cls, ctx, backend.binop_rows(ctx, op, mat[0], vec[0], R, C, vec_first), (R, C))
     x, y = (b[0], a[0]) if reflected else (a[0], b[0])
     return _wrap(cls, ctx, backend.binop(ctx, op, x, y), a[1])
 
 
+def _layout_backend():
+    """K8's hooks run only when the backend has copy_view and binop_view.  CudaBackend always does; a substituted backend
+    without them (a test stand-in) leaves views, joins and broadcasts to the reference's code, as before K8 existed."""
+    return hasattr(backend, 'copy_view') and hasattr(backend, 'binop_view')
+
+
+def _broadcast_binop(cls, ctx, op, operands):
+    """x (op) y under NumPy broadcasting for stores x, y of two shapes (K8's k_binop_view; the broadcast operand is read in
+    place); _MISS for incompatible shapes (NumPy raises) and views beyond the kernels' rank."""
+    (x, sx), (y, sy) = operands
+    if not _layout_backend():
+        return _MISS
+    try:
+        shape, vx, vy = layout.broadcast_views(sx, sy)
+    except ValueError:
+        return _MISS
+    c = layout.collapse(vx, vy)
+    if c is None:
+        return _MISS
+    return _wrap(cls, ctx, backend.binop_view(ctx, op, x, c[0], y, c[1]), shape)
+
+
+def _element(cls, ctx, store):
+    """The field element held by a one-element store (finfields.py:1006-1007 returns elements for 0-d selections)."""
+    calls['limb_ops'] += 1
+    return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, store), ctx)[0]))
+
+
+def _gather(cls, lv, items, out_shape):
+    """A new limb-backed array of out_shape filled by the K8 copies `items` ([(source, src View, dst View)], sources: stores)
+    after collapsing; _MISS when a view has more axes than the kernels take."""
+    n = layout._prod(out_shape)
+    plan = layout.pieces([(i, s, d) for i, (_, s, d) in enumerate(items)])
+    if plan is None:
+        return _MISS
+    store = backend.copy_view(lv.ctx, n, None, [(items[i][0], s, d) for i, s, d in plan])
+    return _wrap(cls, lv.ctx, store, out_shape)
+
+
+def _view_result(cls, lv, view, out_shape):
+    """lv's elements seen through `view`: shares the store when the view is one contiguous run, else one K8 copy."""
+    run = view.run()
+    if run is not None:
+        return cls(LimbValue(lv.ctx, backend.slice(lv.ctx, lv.store, *run), out_shape, lv._poly), check=False)
+    return _gather(cls, lv, [(lv.store, view, layout.View.full(out_shape))], out_shape)
+
+
+def _axis0_run(shape, key):
+    """key is an int (ndim >= 2) or a step-1 slice on axis 0: the contiguous selections that share the store without K8
+    (np_prod's halving loop, runtime.py:2198-2204)."""
+    if isinstance(key, tuple):
+        if len(key) != 1:
+            return False
+        key = key[0]
+    if isinstance(key, slice):
+        return bool(shape) and key.step in (None, 1)
+    return _plain_int(key) and len(shape) >= 2
+
+
 def getitem(self, key):
-    """self[key] for a limb-backed array when the selection is one contiguous run of the C-ordered elements: an int or a
-    step-1 slice along axis 0 (what np_prod's halving loop, runtime.py:2198-2204, and row selections use).  The result
-    shares the limbs (FiniteFieldArray.__getitem__ returns a no-copy view, finfields.py:1004-1009; limb stores are
-    immutable, a later write settles the array that is written to).  _MISS otherwise."""
+    """self[key] for a limb-backed array (FiniteFieldArray.__getitem__, finfields.py:1004-1009) and any key of ints,
+    slices, Ellipsis, None and at most one 1-D integer array (mpyc_b200.layout.getitem_plan).  A selection that is one
+    contiguous run of the C-ordered elements shares the limbs (the reference returns a no-copy view; limb stores are
+    immutable, a later write replaces the store of the array written to); any other covered key is one K8 copy; a 0-d
+    selection is a field element.  _MISS for everything else (boolean masks, several index arrays, keys NumPy rejects),
+    and, on a backend without K8, for every key but an int or step-1 slice on axis 0."""
     cls = type(self)
     lv = as_limb_value(raw_value(self))
     if lv is None:
         return _MISS
-    shape = lv.shape
-    if not shape:
+    plan = layout.getitem_plan(lv.shape, key)
+    if plan is None:
         return _MISS
-    if isinstance(key, tuple):
-        if len(key) != 1:
+    view, out_shape, scalar = plan
+    if not _layout_backend() and not _axis0_run(lv.shape, key):
+        return _MISS
+    if scalar:
+        return _element(cls, lv.ctx, backend.slice(lv.ctx, lv.store, view.offset, view.offset + 1))
+    return _view_result(cls, lv, view, out_shape)
+
+
+def setitem(self, key, value):
+    """self[key] = value (FiniteFieldArray.__setitem__, finfields.py:1011-1029; Runtime.np_update, runtime.py:2657-2679)
+    for a limb-backed array: value is an array of the same class (limb-backed, or of Python ints), a field element or an
+    int, broadcastable to the selection.  The array gets a new store -- a device copy of the old one with the value copied
+    into the selected view (stride 0 on broadcast axes) -- so arrays sharing the old store do not change.  Returns None
+    when done; _MISS leaves the write to the reference (uncovered keys and values, and an index array with repeated
+    entries, whose write order NumPy decides)."""
+    cls = type(self)
+    ctx = _ctx_of(cls)
+    lv = as_limb_value(raw_value(self))
+    if lv is None or ctx is None or lv.ctx is not ctx or not _layout_backend():
+        return _MISS
+    plan = layout.getitem_plan(lv.shape, key)
+    if plan is None:
+        return _MISS
+    view, sel_shape, _ = plan
+    if view.index_axis >= 0 and len(np.unique(view.index)) != len(view.index):
+        return _MISS
+    if isinstance(value, cls):
+        vv = raw_value(value)
+        vlv = as_limb_value(vv)
+        if vlv is not None and vlv.ctx is ctx:
+            vstore, vshape = vlv.store, vlv.shape
+        elif isinstance(vv, np.ndarray) and vv.dtype == object and not ctx.binary:
+            calls['packed'] += 1
+            vstore, vshape = codec.ints_to_limbs(vv.reshape(-1), ctx), vv.shape
+        else:
             return _MISS
-        key = key[0]
-    inner = 1
-    for d in shape[1:]:
-        inner *= d
-    if isinstance(key, slice):
-        if key.step not in (None, 1):
-            return _MISS
-        start, stop, _ = key.indices(shape[0])
-        stop = max(stop, start)
-        new_shape = (stop - start,) + shape[1:]
-    elif isinstance(key, (int, np.integer)) and not isinstance(key, (bool, np.bool_)) and len(shape) >= 2:
-        start = int(key) + (shape[0] if key < 0 else 0)
-        if not 0 <= start < shape[0]:
-            return _MISS                 # NumPy raises the IndexError
-        stop, new_shape = start + 1, shape[1:]
     else:
+        k = _scalar(ctx, cls, value)
+        if k is None:
+            return _MISS
+        vstore, vshape = codec.ints_to_limbs([k if ctx.binary else k % ctx.modulus], ctx), ()
+    try:
+        out, vview, _ = layout.broadcast_views(vshape, sel_shape)
+    except ValueError:
         return _MISS
-    store = backend.slice(lv.ctx, lv.store, start * inner, stop * inner)
-    return cls(LimbValue(lv.ctx, store, new_shape, lv._poly), check=False)
+    if out != sel_shape:
+        return _MISS                      # the value does not broadcast to the selection: the reference raises
+    plan = layout.pieces([(0, vview, view)])
+    if plan is None:
+        return _MISS
+    store = backend.copy_view(ctx, lv.size, lv.store, [(vstore, s, d) for _, s, d in plan])
+    _slot.__set__(self, LimbValue(ctx, store, lv.shape, lv._poly))
+    calls['limb_ops'] += 1
+    return None
+
+
+def permute(self, order):
+    """self.transpose(*axes) / swapaxes / T / np.transpose / np.swapaxes / np.moveaxis for a limb-backed array: `order(ndim)`
+    gives NumPy's axis order (mpyc_b200.layout); one K8 copy, or the shared store when the order moves only length-1 axes.
+    _MISS for bad axes (NumPy raises) and arrays that are not limb-backed."""
+    cls = type(self)
+    lv = as_limb_value(raw_value(self))
+    if lv is None or not _layout_backend():
+        return _MISS
+    try:
+        perm = order(len(lv.shape))
+    except (TypeError, ValueError, IndexError):
+        return _MISS
+    view = layout.permuted(lv.shape, perm)
+    return _view_result(cls, lv, view, view.shape)
+
+
+def _join_parts(cls, arrays):
+    """[(store, shape)] of a join's pieces -- arrays of class cls, limb-backed or (prime fields) of Python ints, which are
+    packed, at least one limb-backed -- or None."""
+    if not isinstance(arrays, (list, tuple)) or not arrays or any(type(a) is not cls for a in arrays):
+        return None
+    ctx = _ctx_of(cls)
+    vals = [raw_value(a) for a in arrays]
+    lvs = [as_limb_value(v) for v in vals]
+    if ctx is None or all(v is None for v in lvs) or any(v is not None and v.ctx is not ctx for v in lvs):
+        return None
+    parts = []
+    for v, x in zip(lvs, vals):
+        if v is not None:
+            parts.append((v.store, v.shape, v._poly))
+        elif isinstance(x, np.ndarray) and x.dtype == object and not ctx.binary:
+            parts.append((None, x.shape, x))
+        else:
+            return None
+    return parts
+
+
+def _pack(ctx, part):
+    store, shape, x = part
+    if store is not None:
+        return store
+    calls['packed'] += 1
+    return codec.ints_to_limbs(x.reshape(-1), ctx)
+
+
+_LAYOUT_PARAMS = {'transpose': ('a', 'axes'), 'swapaxes': ('a', 'axis1', 'axis2'), 'moveaxis': ('a', 'source', 'destination'),
+                  'concatenate': ('arrays', 'axis'), 'stack': ('arrays', 'axis'), 'vstack': ('tup',), 'hstack': ('tup',),
+                  'flip': ('m', 'axis'), 'roll': ('a', 'shift', 'axis'), 'expand_dims': ('a', 'axis'), 'squeeze': ('a', 'axis')}
+_LAYOUT_REQUIRED = {'swapaxes': 3, 'moveaxis': 3, 'roll': 2, 'expand_dims': 2}
+LAYOUT_FUNCTIONS = tuple(getattr(np, name) for name in _LAYOUT_PARAMS)
+
+
+def layout_function(cls, func, args, kwargs):
+    """np.transpose / swapaxes / moveaxis / concatenate / stack / vstack / hstack / flip / roll / expand_dims / squeeze of
+    field arrays (FiniteFieldArray.__array_function__, finfields.py:766-819) on K8: one copy per input (two per rolled
+    axis), or none for expand_dims / squeeze and permutations of length-1 axes, which share the store.  Pieces must be
+    arrays of class cls; anything else (public integer arrays in particular, which the reference reduces), unknown
+    arguments, 0-d results and arguments NumPy rejects give _MISS."""
+    name = func.__name__
+    names = _LAYOUT_PARAMS.get(name)
+    if names is None or len(args) > len(names) or not set(kwargs) <= set(names[len(args):]) or not _layout_backend():
+        return _MISS
+    bound = dict(zip(names, args), **kwargs)
+    if len(bound) < _LAYOUT_REQUIRED.get(name, 1):
+        return _MISS
+    first = bound[names[0]]
+    try:
+        if name in ('concatenate', 'stack', 'vstack', 'hstack'):
+            parts = _join_parts(cls, first)
+            if parts is None:
+                return _MISS
+            shapes = [p[1] for p in parts]
+            if name == 'concatenate':
+                out_shape, items = layout.concatenate_plan(shapes, bound.get('axis', 0))
+            elif name == 'stack':
+                out_shape, items = layout.stack_plan(shapes, bound.get('axis', 0))
+            elif name == 'vstack':
+                out_shape, items = layout.concatenate_plan(layout.vstack_shapes(shapes), 0)
+            else:
+                out_shape, items = layout.concatenate_plan(*layout.hstack_axis(shapes))
+            if not out_shape:
+                return _MISS
+            ctx = _ctx_of(cls)
+            stores = [_pack(ctx, p) for p in parts]
+            poly = next(p[2] for p in parts if p[0] is not None)
+            lv = LimbValue(ctx, stores[0], shapes[0], poly)
+            return _gather(cls, lv, [(stores[i], s, d) for i, s, d in items], out_shape)
+        if type(first) is not cls:
+            return _MISS
+        lv = as_limb_value(raw_value(first))
+        if lv is None:
+            return _MISS
+        shape = lv.shape
+        if name in ('transpose', 'swapaxes', 'moveaxis'):
+            if name == 'transpose':
+                return permute(first, lambda nd: layout.transpose_axes(nd, (bound.get('axes'),)))
+            if name == 'swapaxes':
+                return permute(first, lambda nd: layout.swapaxes_axes(nd, bound['axis1'], bound['axis2']))
+            return permute(first, lambda nd: layout.moveaxis_axes(nd, bound['source'], bound['destination']))
+        if name in ('expand_dims', 'squeeze'):
+            out_shape = layout.reshaped(shape, func, bound.get('axis'))
+            if not out_shape:
+                return _MISS
+            return cls(LimbValue(lv.ctx, lv.store, out_shape, lv._poly), check=False)
+        if not shape:
+            return _MISS
+        if name == 'flip':
+            view = layout.flip_view(shape, bound.get('axis'))
+            return _view_result(cls, lv, view, shape)
+        shift, axis = bound['shift'], bound.get('axis')
+        if not _plain_int(shift) or not (axis is None or _plain_int(axis)):
+            return _MISS
+        return _gather(cls, lv, [(lv.store, s, d) for _, s, d in layout.roll_plan(shape, int(shift), axis)], shape)
+    except (TypeError, ValueError, IndexError):
+        return _MISS
 
 
 def concatenate(cls, arrays, axis):

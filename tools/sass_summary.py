@@ -37,7 +37,7 @@ def main():
     pats = sys.argv[1:] or DEFAULT
     rows = []
     for obj in sorted(glob.glob(os.path.join(OBJ, '*.o'))):
-        if not obj.endswith(('api.o', 'inst_L1.o', 'inst_L2.o', 'inst_L3.o', 'inst_L4.o')):
+        if not obj.endswith(('api.o', 'inst_L1.o', 'inst_L2.o', 'inst_L3.o', 'inst_L4.o', 'inst_layout.o')):
             continue
         sass = subprocess.run(['cuobjdump', '-sass', obj], capture_output=True, text=True).stdout
         res = subprocess.run(['cuobjdump', '-res-usage', obj], capture_output=True, text=True).stdout
