@@ -190,6 +190,22 @@ int mpyc_b200_copy_view(size_t elem_bytes, const void* d_src, size_t src_len, co
 int mpyc_b200_ff_binop_view(const mpyc_b200_field* f, int op, const void* d_a, size_t a_len, const mpyc_b200_view* a,
                             const void* d_b, size_t b_len, const mpyc_b200_view* b, void* d_out, void* stream);
 
+/* ---- determinants, linear solves and inverses (K9) ----------------------------------------------
+ * Prime fields; matrices are dense, row-major, elements contiguous.  Inputs are never modified (the elimination runs on
+ * a stream-ordered workspace copy).  Both entry points reject sizes whose byte counts overflow, n == 0 and an output that
+ * overlaps an input with MPYC_B200_EINVAL before any CUDA call.
+ *
+ * d_out[b] = det of the n x n matrix b of d_a (batch x n x n), as FiniteFieldArray.gauss_det computes it
+ * (mpyc/finfields.py:916-955): Gaussian elimination that swaps row k with the first row below it with a nonzero entry
+ * in column k when a[k][k] == 0, and does NOT negate the result for a swap; 0 for a singular matrix.  np.linalg.det and
+ * Runtime.np_det (mpyc/runtime.py:3951-3982). */
+int mpyc_b200_ff_det(const mpyc_b200_field* f, const void* d_a, size_t batch, size_t n, void* d_out, void* stream);
+/* d_x (n x nrhs) = d_a^-1 d_b for d_a n x n and d_b n x nrhs; d_b == NULL means the identity (nrhs must be n), which gives
+ * the inverse.  gauss_solve / gauss_inv (mpyc/finfields.py:872-914): np.linalg.solve / inv.  Synchronises the stream;
+ * MPYC_B200_EZERODIV ("no inverse exists") when d_a is singular, d_x is then undefined. */
+int mpyc_b200_ff_solve(const mpyc_b200_field* f, const void* d_a, size_t n, const void* d_b, size_t nrhs, void* d_x,
+                       void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -873,6 +873,45 @@ MPYC_API int mpyc_b200_ff_binop_view(const mpyc_b200_field* f, int op, const voi
     });
 }
 
+// ---------------------------------------------------------------------------------------
+// K9: determinants, solves and inverses (linalg.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+MPYC_API int mpyc_b200_ff_det(const mpyc_b200_field* f, const void* d_a, size_t batch, size_t n, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_det: field is null")) return rc;
+    if (n == 0) return fail(MPYC_B200_EINVAL, "ff_det: n must be at least 1");
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t ab = 0, ob = 0;
+    if (__builtin_mul_overflow(n, n, &ab) || __builtin_mul_overflow(ab, batch, &ab) || __builtin_mul_overflow(ab, E, &ab) ||
+        __builtin_mul_overflow(batch, E, &ob))
+        return fail(MPYC_B200_EINVAL, "ff_det: size overflow");
+    if (batch == 0) return MPYC_B200_OK;
+    if (!d_a || !d_out) return fail(MPYC_B200_EINVAL, "ff_det: null buffer");
+    if (bytes_overlap(d_a, ab, d_out, ob)) return fail(MPYC_B200_EINVAL, "ff_det: out overlaps the matrices");
+    return launch_status(launch_det(f->fp, (const u64*)d_a, batch, n, (u64*)d_out, (cudaStream_t)stream), "ff_det launch");
+}
+
+MPYC_API int mpyc_b200_ff_solve(const mpyc_b200_field* f, const void* d_a, size_t n, const void* d_b, size_t nrhs, void* d_x,
+                                void* stream) {
+    if (int rc = prime_only(f, "ff_solve: field is null")) return rc;
+    if (n == 0) return fail(MPYC_B200_EINVAL, "ff_solve: n must be at least 1");
+    if (!d_b && nrhs != n) return fail(MPYC_B200_EINVAL, "ff_solve: the identity right-hand side has n columns");
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t ab = 0, bb = 0, w = 0;
+    if (__builtin_mul_overflow(n, n, &ab) || __builtin_mul_overflow(ab, E, &ab) || __builtin_mul_overflow(n, nrhs, &bb) ||
+        __builtin_mul_overflow(bb, E, &bb) || __builtin_add_overflow(n, nrhs, &w) || __builtin_mul_overflow(w, n, &w) ||
+        __builtin_mul_overflow(w, E, &w))
+        return fail(MPYC_B200_EINVAL, "ff_solve: size overflow");
+    if (!d_a || (nrhs && !d_x)) return fail(MPYC_B200_EINVAL, "ff_solve: null buffer");
+    if (bytes_overlap(d_x, bb, d_a, ab) || (d_b && bytes_overlap(d_x, bb, d_b, bb)))
+        return fail(MPYC_B200_EINVAL, "ff_solve: x overlaps an operand");
+    int singular = 0;
+    const int rc = launch_status(launch_solve(f->fp, (const u64*)d_a, n, (const u64*)d_b, nrhs, (u64*)d_x, &singular,
+                                              (cudaStream_t)stream), "ff_solve launch");
+    if (rc != MPYC_B200_OK) return rc;
+    return singular ? fail(MPYC_B200_EZERODIV, "no inverse exists") : MPYC_B200_OK;
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

@@ -86,6 +86,14 @@ struct Launch {
 // their index tables (if any) are in device memory
 cudaError_t launch_copy_view(const CopyPlan& pl, size_t elem_bytes, const void* src, void* dst, cudaStream_t st);
 
+// K9 (inst_linalg.cu): out[b] = det of the n x n matrix b of a (batch x n x n; the reference's determinant, which ignores
+// the sign of its row swaps).  Prime fields; sizes validated by the caller.
+cudaError_t launch_det(const FieldParams& fp, const u64* a, size_t batch, size_t n, u64* out, cudaStream_t st);
+// x (n x nrhs) = a^-1 b, b null: the identity (nrhs = n).  Synchronises st; *singular = 1 when a has no inverse (x is
+// then undefined).
+cudaError_t launch_solve(const FieldParams& fp, const u64* a, size_t n, const u64* b, size_t nrhs, u64* x, int* singular,
+                         cudaStream_t st);
+
 extern template struct Launch<1>;
 extern template struct Launch<2>;
 extern template struct Launch<3>;

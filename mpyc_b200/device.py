@@ -515,6 +515,59 @@ def binop_view(a: DeviceArray, a_view, b: DeviceArray, b_view, op):
     return out
 
 
+# ---- K9: determinants, solves, inverses and powers of matrices (csrc/linalg.cuh) ------------------------------------
+
+def det(a: DeviceArray, batch, n):
+    """det of each n x n matrix of a (batch x n x n, row-major) as FiniteFieldArray.gauss_det computes it: row swaps do not
+    change the sign (mpyc/finfields.py:916-955).  A DeviceArray of batch elements."""
+    _check_elements(a, (batch, n, n), 'det')
+    out = DeviceArray.empty(a.ctx, batch, a.t.device)
+    check(lib.mpyc_b200_ff_det(a.ctx.handle, a.ptr, batch, n, out.ptr, _stream_ptr()))
+    return out
+
+
+def solve(a: DeviceArray, b, n, nrhs):
+    """X (n x nrhs) with a X = b for a (n x n) and b (n x nrhs); b None: the inverse of a (nrhs = n).  ZeroDivisionError('no
+    inverse exists') for a singular a (gauss_solve / gauss_inv, mpyc/finfields.py:872-914)."""
+    _check_elements(a, (n, n), 'solve')
+    if b is not None:
+        if b.ctx is not a.ctx:
+            raise ValueError('solve: arrays of different fields')
+        _check_elements(b, (n, nrhs), 'solve')
+    elif nrhs != n:
+        raise ValueError('solve: the identity right-hand side has n columns')
+    out = DeviceArray.empty(a.ctx, n * nrhs, a.t.device)
+    check(lib.mpyc_b200_ff_solve(a.ctx.handle, a.ptr, n, b.ptr if b is not None else ctypes.c_void_p(0), nrhs, out.ptr,
+                                 _stream_ptr()))
+    return out
+
+
+def inv(a: DeviceArray, n):
+    return solve(a, None, n, n)
+
+
+def identity(ctx, n, device='cuda'):
+    e = DeviceArray(ctx, torch.zeros((n * n, ctx.nlimbs), dtype=torch.int64, device=device))
+    e.t[::n + 1, 0] = 1
+    return e
+
+
+def matrix_power(a: DeviceArray, n, e):
+    """a^e for an n x n matrix a and a Python int e: square and multiply on K1c (matrix_pow, mpyc/finfields.py:957-976);
+    the inverse first for e < 0 (ZeroDivisionError for a singular a), the identity for e == 0."""
+    _check_elements(a, (n, n), 'matrix_power')
+    if e < 0:
+        a, e = inv(a, n), -e
+    c = None
+    while e:
+        if e & 1:
+            c = a if c is None else matmul(a.ctx, c, a, n, n, n)
+        e >>= 1
+        if e:
+            a = matmul(a.ctx, a, a, n, n, n)
+    return identity(a.ctx, n, a.t.device) if c is None else c
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

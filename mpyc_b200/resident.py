@@ -179,6 +179,20 @@ class CudaBackend:
         dev, _ = self._dev()
         return dev.binop_view(self.to_store(ctx, a), a_view, self.to_store(ctx, b), b_view, op)
 
+    def det(self, ctx, a, batch, n):
+        """store of the batch determinants of a (batch x n x n) (K9)"""
+        dev, _ = self._dev()
+        return dev.det(self.to_store(ctx, a), batch, n)
+
+    def solve(self, ctx, a, n, b, nrhs):
+        """store of X (n x nrhs) with a X = b; b None: the inverse of a.  ZeroDivisionError for a singular a (K9)"""
+        dev, _ = self._dev()
+        return dev.solve(self.to_store(ctx, a), None if b is None else self.to_store(ctx, b), n, nrhs)
+
+    def matrix_power(self, ctx, a, n, e):
+        dev, _ = self._dev()
+        return dev.matrix_power(self.to_store(ctx, a), n, e)
+
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
         return dev.conv2d(self.to_store(ctx, X), self.to_store(ctx, W), self.to_store(ctx, B), k, r, m, n, v, s)
@@ -1519,6 +1533,77 @@ def array_function(self, func, args, kwargs):
     if axis is None and np.ndim(raw_value(first)) > 1:
         return _MISS                      # NumPy requires the axis of a multi-dimensional array
     return cumsum(first, axis, bool(opt('include_initial', False)))
+
+
+# the parameter names of the reference's implementations, so that keywords it rejects stay with it
+_LINALG_PARAMS = {'det': ('a',), 'solve': ('A', 'B'), 'inv': ('A',), 'matrix_power': ('A', 'n')}
+LINALG_FUNCTIONS = tuple(getattr(np.linalg, name) for name in _LINALG_PARAMS)
+
+
+def _linalg_backend():
+    """K9's hooks run only when the backend has det and solve (and matrix_power for np.linalg.matrix_power).  CudaBackend
+    always does; a substituted backend without them (a test stand-in) leaves linear algebra to the reference's code."""
+    return hasattr(backend, 'det') and hasattr(backend, 'solve')
+
+
+def linalg_function(cls, func, args, kwargs):
+    """np.linalg.det / solve / inv / matrix_power of prime-field arrays (FiniteFieldArray.gauss_det / gauss_solve /
+    gauss_inv / matrix_pow, finfields.py:872-976) on K9 and K1c.  det: a field element for one matrix, a limb-backed array
+    of shape a.shape[:-2] for a stack; solve / inv / matrix_power: a limb-backed (n, m) array.  Operands must be arrays of
+    class cls, limb-backed or of at least min_size elements (both are packed once one qualifies, as for @).  _MISS, so that
+    the reference raises its own errors, for: non-square or ndim < 2 operands, n == 0 or empty stacks, stacked solve / inv /
+    matrix_power, a b that is not a 2-D array of cls with n rows, an exponent that is not a Python int, binary fields and
+    unknown arguments."""
+    name = func.__name__
+    names = _LINALG_PARAMS[name]
+    if len(args) > len(names) or not set(kwargs) <= set(names[len(args):]) or not _linalg_backend():
+        return _MISS
+    bound = dict(zip(names, args), **kwargs)
+    if len(bound) != len(names):
+        return _MISS
+    ctx = _ctx_of(cls)
+    A, B = bound[names[0]], bound.get('B')
+    if ctx is None or ctx.binary or type(A) is not cls:
+        return _MISS
+    shape = getattr(raw_value(A), 'shape', None)
+    if shape is None or len(shape) < 2 or shape[-1] != shape[-2] or shape[-1] == 0 or (name != 'det' and len(shape) != 2):
+        return _MISS
+    n = shape[-1]
+    batch = layout._prod(shape[:-2])
+    if batch == 0:
+        return _MISS
+    operands = [A]
+    if name == 'solve':
+        sb = getattr(raw_value(B), 'shape', None) if type(B) is cls else None
+        if sb is None or len(sb) != 2 or sb[0] != n or sb[1] == 0:
+            return _MISS
+        operands.append(B)
+    elif name == 'matrix_power' and (type(bound['n']) is not int or not hasattr(backend, 'matrix_power')):
+        return _MISS
+    limbish = any(as_limb_value(raw_value(x)) is not None for x in operands)
+    if not limbish and np.size(raw_value(A)) < min_size:
+        return _MISS
+    saved = min_size
+    try:
+        globals()['min_size'] = 0         # both operands are packed whatever their size
+        ops = [_operand(ctx, cls, x) for x in operands]
+    finally:
+        globals()['min_size'] = saved
+    if any(o is None for o in ops):
+        return _MISS
+    a = ops[0][0]
+    if name == 'det':
+        out = backend.det(ctx, a, batch, n)
+        if len(shape) == 2:
+            calls['limb_ops'] += 1
+            return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
+        return _wrap(cls, ctx, out, shape[:-2])
+    if name == 'solve':
+        nrhs = ops[1][1][1]
+        return _wrap(cls, ctx, backend.solve(ctx, a, n, ops[1][0], nrhs), (n, nrhs))
+    if name == 'inv':
+        return _wrap(cls, ctx, backend.solve(ctx, a, n, None, n), (n, n))
+    return _wrap(cls, ctx, backend.matrix_power(ctx, a, n, bound['n']), (n, n))
 
 
 def conv2d(x, W, b):
