@@ -206,6 +206,16 @@ int mpyc_b200_ff_det(const mpyc_b200_field* f, const void* d_a, size_t batch, si
 int mpyc_b200_ff_solve(const mpyc_b200_field* f, const void* d_a, size_t n, const void* d_b, size_t nrhs, void* d_x,
                        void* stream);
 
+/* ---- 1-D convolution (K10) ----------------------------------------------------------------------
+ * d_c[j] = sum_{i + l = lo + j} a[i] * b[l] mod p for j < count (np.convolve, finfields.py:766-819; Runtime.np_convolve,
+ * runtime.py:2580-2634; the secret-shift branch of Runtime.np_roll, runtime.py:3300-3314).  Prime fields.  The window
+ * [lo, lo + count) of the full result (m + n - 1 elements) is computed alone: np.convolve's 'full' is lo = 0,
+ * count = m + n - 1; with s = min(m, n), g = max(m, n), 'same' is lo = (s - 1) / 2, count = g and 'valid' is lo = s - 1,
+ * count = g - s + 1.  Any 8-byte aligned buffers work.  MPYC_B200_EINVAL before any CUDA call for m == 0 or n == 0,
+ * lo + count > m + n - 1, byte counts that overflow and an output that overlaps an input; count == 0 does nothing. */
+int mpyc_b200_ff_convolve(const mpyc_b200_field* f, const void* d_a, size_t m, const void* d_b, size_t n,
+                          size_t lo, size_t count, void* d_c, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

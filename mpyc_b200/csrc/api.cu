@@ -912,6 +912,28 @@ MPYC_API int mpyc_b200_ff_solve(const mpyc_b200_field* f, const void* d_a, size_
     return singular ? fail(MPYC_B200_EZERODIV, "no inverse exists") : MPYC_B200_OK;
 }
 
+// ---------------------------------------------------------------------------------------
+// K10: 1-D convolution (conv.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+MPYC_API int mpyc_b200_ff_convolve(const mpyc_b200_field* f, const void* d_a, size_t m, const void* d_b, size_t n, size_t lo,
+                                   size_t count, void* d_c, void* stream) {
+    if (int rc = prime_only(f, "ff_convolve: field is null")) return rc;
+    if (m == 0 || n == 0) return fail(MPYC_B200_EINVAL, "ff_convolve: empty operand");
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t full = 0, end = 0, ab = 0, bb = 0, cb = 0;
+    if (__builtin_add_overflow(m, n - 1, &full) || __builtin_add_overflow(lo, count, &end) || __builtin_mul_overflow(m, E, &ab) ||
+        __builtin_mul_overflow(n, E, &bb) || __builtin_mul_overflow(count, E, &cb) || full > (size_t)INT64_MAX / E)
+        return fail(MPYC_B200_EINVAL, "ff_convolve: size overflow");
+    if (end > full) return fail(MPYC_B200_EINVAL, "ff_convolve: window past the full result");
+    if (count == 0) return MPYC_B200_OK;
+    if (!d_a || !d_b || !d_c) return fail(MPYC_B200_EINVAL, "ff_convolve: null buffer");
+    if (bytes_overlap(d_c, cb, d_a, ab) || bytes_overlap(d_c, cb, d_b, bb))
+        return fail(MPYC_B200_EINVAL, "ff_convolve: c overlaps an operand");
+    return launch_status(launch_convolve(f->fp, (const u64*)d_a, m, (const u64*)d_b, n, lo, count, (u64*)d_c, (cudaStream_t)stream),
+                         "ff_convolve launch");
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

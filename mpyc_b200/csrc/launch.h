@@ -94,6 +94,11 @@ cudaError_t launch_det(const FieldParams& fp, const u64* a, size_t batch, size_t
 cudaError_t launch_solve(const FieldParams& fp, const u64* a, size_t n, const u64* b, size_t nrhs, u64* x, int* singular,
                          cudaStream_t st);
 
+// K10 (inst_conv.cu): c[j] = sum_{i + l = lo + j} a[i] b[l] mod p for j < count (a of m, b of n elements).  Prime fields;
+// sizes validated by the caller.
+cudaError_t launch_convolve(const FieldParams& fp, const u64* a, size_t m, const u64* b, size_t n, size_t lo, size_t count,
+                            u64* c, cudaStream_t st);
+
 extern template struct Launch<1>;
 extern template struct Launch<2>;
 extern template struct Launch<3>;

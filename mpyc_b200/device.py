@@ -568,6 +568,21 @@ def matrix_power(a: DeviceArray, n, e):
     return identity(a.ctx, n, a.t.device) if c is None else c
 
 
+# ---- K10: 1-D convolution (csrc/conv.cuh) ------------------------------------------------------------------------
+
+def convolve(ctx, a: DeviceArray, m, b: DeviceArray, n, lo, count):
+    """c[j] = sum_{i + l = lo + j} a[i] b[l] mod p for j < count: the window [lo, lo + count) of np.convolve(a, b)
+    (m + n - 1 elements), computed alone (np.convolve of field arrays, mpyc/finfields.py:766-819).  A DeviceArray of
+    count elements."""
+    if a.ctx is not ctx or b.ctx is not ctx:
+        raise ValueError('convolve: arrays of different fields')
+    _check_elements(a, (m,), 'convolve')
+    _check_elements(b, (n,), 'convolve')
+    out = DeviceArray.empty(ctx, count, a.t.device)
+    check(lib.mpyc_b200_ff_convolve(ctx.handle, a.ptr, m, b.ptr, n, lo, count, out.ptr, _stream_ptr()))
+    return out
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

@@ -116,7 +116,7 @@ def _install_operators(finfields_module, min_size):
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
     np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays.  Views, writes,
     axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
-    np.linalg.det / solve / inv / matrix_power on K9 and K1c; everything else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
+    np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10; everything else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
     from mpyc_b200 import _cabi, resident
     resident.min_size = int(min_size)
     cls = finfields_module.FiniteFieldArray
@@ -210,6 +210,10 @@ def _install_operators(finfields_module, min_size):
                 return r
         if func in resident.LINALG_FUNCTIONS and isinstance(self, cls):
             r = resident.linalg_function(type(self), func, args, kwargs)
+            if r is not MISS:
+                return r
+        if func is np.convolve and isinstance(self, cls):
+            r = resident.convolve(type(self), args, kwargs)
             if r is not MISS:
                 return r
         return orig['__array_function__'](self, func, types, args, kwargs)

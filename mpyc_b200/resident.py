@@ -193,6 +193,11 @@ class CudaBackend:
         dev, _ = self._dev()
         return dev.matrix_power(self.to_store(ctx, a), n, e)
 
+    def convolve(self, ctx, a, m, b, n, lo, count):
+        """store of full[lo : lo + count] of the convolution of a (m) and b (n) (K10)"""
+        dev, _ = self._dev()
+        return dev.convolve(ctx, self.to_store(ctx, a), m, self.to_store(ctx, b), n, lo, count)
+
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
         return dev.conv2d(self.to_store(ctx, X), self.to_store(ctx, W), self.to_store(ctx, B), k, r, m, n, v, s)
@@ -1604,6 +1609,80 @@ def linalg_function(cls, func, args, kwargs):
     if name == 'inv':
         return _wrap(cls, ctx, backend.solve(ctx, a, n, None, n), (n, n))
     return _wrap(cls, ctx, backend.matrix_power(ctx, a, n, bound['n']), (n, n))
+
+
+def _public_ints(x):
+    """The entries of a public 1-D integer operand of np.convolve as a list of Python ints: a list, tuple or range of
+    ints, an integer-dtype ndarray or an object ndarray of Python ints.  None for anything else (floats, bools, field
+    elements, other dimensions)."""
+    if isinstance(x, range):
+        return list(x)
+    if isinstance(x, (list, tuple)):
+        return list(x) if all(type(e) is int for e in x) else None
+    if isinstance(x, np.ndarray) and x.ndim == 1:
+        if x.dtype.kind in 'iu':
+            return [int(e) for e in x.tolist()]
+        if x.dtype == object and all(type(e) is int for e in x):
+            return x.tolist()
+    return None
+
+
+_CONVOLVE_MODES = ('full', 'same', 'valid')
+
+
+def convolve(cls, args, kwargs):
+    """np.convolve(a, v, mode) of prime-field vectors (FiniteFieldArray.__array_function__, finfields.py:766-819; the local
+    step of Runtime.np_convolve and of np_roll's secret shift) on K10: a limb-backed array of cls holding the window of
+    the full result that mode selects.  One operand is a 1-D array of cls; the other is one too, or a public integer
+    sequence (_public_ints), whose entries are reduced mod p and packed -- exact, as convolution is bilinear and the
+    reference's cls(result) reduces.  Both are packed once one operand is limb-backed or m * n >= min_size, as for
+    np.outer.  _MISS, so that the reference keeps its own results and errors, for: binary or uncovered fields, operands
+    that are 0-d, field elements, empty or not 1-D, other dtypes, arrays of another field, modes other than the three
+    strings, operands passed by keyword, unknown arguments and a backend without convolve."""
+    if not 2 <= len(args) <= 3 or not set(kwargs) <= ({'mode'} if len(args) == 2 else set()) or not hasattr(backend, 'convolve'):
+        return _MISS                      # operands by keyword: the reference recurses (it unpacks positional ones only)
+    mode = args[2] if len(args) == 3 else kwargs.get('mode', 'full')
+    if type(mode) is not str or mode not in _CONVOLVE_MODES:
+        return _MISS
+    ctx = _ctx_of(cls)
+    if ctx is None or ctx.binary:
+        return _MISS
+    operands = list(args[:2])
+    if not any(type(x) is cls for x in operands):
+        return _MISS
+    sizes, public, limbish = [], [None, None], False
+    for k, x in enumerate(operands):
+        if type(x) is cls:
+            shape = getattr(raw_value(x), 'shape', None)
+            limbish = limbish or as_limb_value(raw_value(x)) is not None
+        else:
+            public[k] = _public_ints(x)
+            shape = None if public[k] is None else (len(public[k]),)
+        if shape is None or len(shape) != 1 or shape[0] == 0:
+            return _MISS
+        sizes.append(shape[0])
+    m, n = sizes
+    if not limbish and m * n < min_size:
+        return _MISS
+    stores = [None, None]
+    saved = min_size
+    try:
+        globals()['min_size'] = 0         # both operands are packed whatever their size
+        for k, x in enumerate(operands):
+            if public[k] is None:
+                op = _operand(ctx, cls, x)
+                if op is None:
+                    return _MISS
+                stores[k] = op[0]
+    finally:
+        globals()['min_size'] = saved
+    for k, ints in enumerate(public):
+        if ints is not None:
+            calls['packed'] += 1
+            stores[k] = codec.ints_to_limbs([e % ctx.modulus for e in ints], ctx)
+    s, g = min(m, n), max(m, n)
+    lo, count = {'full': (0, m + n - 1), 'same': ((s - 1) // 2, g), 'valid': (s - 1, g - s + 1)}[mode]
+    return _wrap(cls, ctx, backend.convolve(ctx, stores[0], m, stores[1], n, lo, count), (count,))
 
 
 def conv2d(x, W, b):
