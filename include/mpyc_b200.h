@@ -216,6 +216,23 @@ int mpyc_b200_ff_solve(const mpyc_b200_field* f, const void* d_a, size_t n, cons
 int mpyc_b200_ff_convolve(const mpyc_b200_field* f, const void* d_a, size_t m, const void* d_b, size_t n,
                           size_t lo, size_t count, void* d_c, void* stream);
 
+/* ---- division and selection (K11) ---------------------------------------------------------------
+ * d_out[h] = d_num[h] * d_den[h]^-1 mod p in one Montgomery-trick pass (FiniteFieldArray.__truediv__ / __itruediv__,
+ * finfields.py:1199-1225, whose `self.value * cls._reciprocal(other)` it replaces; Runtime.np_reciprocal's `r / ar`,
+ * runtime.py:1290).  Prime fields.  MPYC_B200_EZERODIV if any d_den[h] == 0 (synchronises the stream, as ff_inv).
+ * MPYC_B200_EINVAL before any CUDA call for null buffers, byte counts that overflow and an output that overlaps either
+ * input (the forward pass keeps prefix products in d_out); num and den may be the same buffer. */
+int mpyc_b200_ff_div(const mpyc_b200_field* f, const void* d_num, const void* d_den, void* d_out, size_t n, void* stream);
+
+/* d_out[h] = ((d_mask[h] != 0) != invert) ? X(h) : Y(h) mod p: np.where(cond, x, y) of field arrays and raw share values
+ * (finfields.py:766-819; Runtime._np_is_zero, runtime.py:3614-3615; Runtime.np_lsb, runtime.py:1819).  A side is
+ * d_x[h] * s + t with h_x_st = {s (L limbs), t (L limbs)}, canonical residues, or the constant t when d_x is null (likewise
+ * Y).  d_mask: n bytes in device memory.  Element buffers need 8-byte alignment only.  Prime fields; MPYC_B200_EINVAL
+ * before any CUDA call for null buffers or maps, non-canonical scalars, byte counts that overflow and an output that
+ * overlaps an input. */
+int mpyc_b200_ff_select(const mpyc_b200_field* f, const uint8_t* d_mask, int invert, const void* d_x, const uint64_t* h_x_st,
+                        const void* d_y, const uint64_t* h_y_st, void* d_out, size_t n, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -934,6 +934,65 @@ MPYC_API int mpyc_b200_ff_convolve(const mpyc_b200_field* f, const void* d_a, si
                          "ff_convolve launch");
 }
 
+// ---------------------------------------------------------------------------------------
+// K11: division (k_inv_batch with a numerator) and selection (select.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+MPYC_API int mpyc_b200_ff_div(const mpyc_b200_field* f, const void* d_num, const void* d_den, void* d_out, size_t n,
+                              void* stream) {
+    if (int rc = prime_only(f, "ff_div: field is null")) return rc;
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t bytes = 0;
+    if (__builtin_mul_overflow(n, E, &bytes) || bytes > (size_t)INT64_MAX) return fail(MPYC_B200_EINVAL, "ff_div: size overflow");
+    if (n == 0) return MPYC_B200_OK;
+    if (!d_num || !d_den || !d_out) return fail(MPYC_B200_EINVAL, "ff_div: null buffer");
+    // the forward pass leaves prefix products in out, which the backward pass reads next to num and den
+    if (bytes_overlap(d_out, bytes, d_num, bytes) || bytes_overlap(d_out, bytes, d_den, bytes))
+        return fail(MPYC_B200_EINVAL, "ff_div: out overlaps an operand");
+    cudaStream_t st = (cudaStream_t)stream;
+    u64 e[4];
+    wide_copy(e, f->fp.p, 4);
+    wide_sub_small(e, 4, 2);   // p - 2
+    ExpParams ex;
+    memset(&ex, 0, sizeof ex);
+    for (int i = 0; i < 4; i++) ex.e[i] = e[i];
+    ex.ebits = bit_length(ex.e, 8);
+    ZeroFlag zf;
+    if (int zrc = zf.acquire(st)) return zrc;
+    int rc = with_limbs((int)f->fp.L, [&](auto Lc) {
+        constexpr int L = decltype(Lc)::value;
+        return launch_status(Launch<L>::inv_batch(f->fp, ex, (const u64*)d_den, (u64*)d_out, zf.d, n, st, (const u64*)d_num),
+                             "ff_div launch");
+    });
+    if (rc != MPYC_B200_OK) return rc;
+    int flag = 0;
+    CU(cudaMemcpyAsync(&flag, zf.d, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return flag ? fail(MPYC_B200_EZERODIV, "inverse of zero") : MPYC_B200_OK;
+}
+
+MPYC_API int mpyc_b200_ff_select(const mpyc_b200_field* f, const uint8_t* d_mask, int invert, const void* d_x,
+                                 const uint64_t* h_x_st, const void* d_y, const uint64_t* h_y_st, void* d_out, size_t n,
+                                 void* stream) {
+    if (int rc = prime_only(f, "ff_select: field is null")) return rc;
+    if (!h_x_st || !h_y_st) return fail(MPYC_B200_EINVAL, "ff_select: null affine map");
+    const size_t L = f->fp.L, E = L * sizeof(u64);
+    for (const uint64_t* m : {h_x_st, h_y_st})
+        if (!canonical(f, m) || !canonical(f, m + L)) return fail(MPYC_B200_EINVAL, "ff_select: scalars must be canonical residues");
+    size_t bytes = 0;
+    if (__builtin_mul_overflow(n, E, &bytes) || bytes > (size_t)INT64_MAX) return fail(MPYC_B200_EINVAL, "ff_select: size overflow");
+    if (n == 0) return MPYC_B200_OK;
+    if (!d_mask || !d_out) return fail(MPYC_B200_EINVAL, "ff_select: null buffer");
+    if (bytes_overlap(d_out, bytes, d_mask, n) || (d_x && bytes_overlap(d_out, bytes, d_x, bytes)) ||
+        (d_y && bytes_overlap(d_out, bytes, d_y, bytes)))
+        return fail(MPYC_B200_EINVAL, "ff_select: out overlaps an operand");
+    const u64* xst = (const u64*)h_x_st;
+    const u64* yst = (const u64*)h_y_st;
+    return launch_status(launch_select(f->fp, d_mask, invert != 0, (const u64*)d_x, xst, xst + L, (const u64*)d_y, yst, yst + L,
+                                       (u64*)d_out, n, (cudaStream_t)stream),
+                         "ff_select launch");
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

@@ -16,6 +16,7 @@
 //   K4   k_prss_tiles, k_prss_combine           thresha.py:163-173,201-217
 //   K7   k_sum_cols / k_sum_rows, k_scan_cols / k_scan_rows (reduce.cuh)   np.sum / np.cumsum along any axis
 //   K8   k_copy_gather, k_copy_permute, k_binop_view (layout.cuh)   strided views, joins, broadcast arithmetic
+//   K11  k_inv_batch<NUM> (ff_div), k_select (select.cuh)   division and np.where       finfields.py:1199-1225
 #pragma once
 #include "ff_arith.cuh"
 
@@ -246,6 +247,9 @@ k_pow(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* __restrict__ 
 // i.e. 3 multiplications per element + 1/B of an exponentiation (~1.5 bits(p) multiplications) instead of
 // a whole one.  Zeros are skipped in the products (the result for them is 0) and reported through
 // zero_flag (the reference raises ZeroDivisionError, gmpy.py:192-213).  a and out must not alias.
+// NUM (K11, ff_div): the backward walk multiplies each inverse by num[h] before storing it, so that
+// out[h] = num[h] * a[h]^-1 in the same pass -- one more load and one more multiplication per element.  num may
+// alias a but not out (the forward pass leaves prefix products in out).  Without NUM, num is unused.
 // ---------------------------------------------------------------------------------------
 
 template <int L>
@@ -258,9 +262,10 @@ __device__ __forceinline__ void load_plain(u32* v, const u64* p) {   // coherent
     }
 }
 
-template <int L, int KIND>
+template <int L, int KIND, bool NUM = false>
 __global__ void MPYC_LB
-k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, int* zero_flag, size_t n, size_t T, int B) {
+k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, int* zero_flag, size_t n, size_t T, int B,
+            const u64* __restrict__ num) {
     typedef Fp<L, KIND> F;
     constexpr int N = 2 * L;
     const size_t nth = (size_t)gridDim.x * blockDim.x;
@@ -300,6 +305,11 @@ k_inv_batch(FieldParams f, ExpParams ex, const u64* __restrict__ a, u64* out, in
                 copy_n<N>(r, inv);
             }
             F::mul(inv, inv, x, f);
+            if constexpr (NUM) {
+                u32 y[N];
+                load_limbs<L, false>(y, num + h * L);
+                F::mul(r, r, y, f);
+            }
             if (z) zero_n<N>(r);
             store_limbs<L, false>(out + h * L, r);
         }

@@ -26,9 +26,10 @@ struct Launch {
     // mode 0: out = a^e; mode 1: out8 = (a^e != p-1)
     static cudaError_t pow(const FieldParams& fp, const ExpParams& ex, int mode, const u64* a, u64* out,
                            unsigned char* out8, int* zero_flag, size_t n, cudaStream_t st);
-    // out[h] = a[h]^-1 (0 for a[h] == 0, reported in zero_flag); ex = p - 2; a and out must not alias
+    // out[h] = a[h]^-1 (0 for a[h] == 0, reported in zero_flag); ex = p - 2; a and out must not alias.
+    // num (K11): out[h] = num[h] * a[h]^-1 in the same pass; num must not alias out
     static cudaError_t inv_batch(const FieldParams& fp, const ExpParams& ex, const u64* a, u64* out, int* zero_flag,
-                                 size_t n, cudaStream_t st);
+                                 size_t n, cudaStream_t st, const u64* num = nullptr);
     static cudaError_t split(const FieldParams& fp, bool full, const u64* secrets, const u64* coeffs, size_t cstride,
                              u64* shares, size_t sstride, size_t n, int t, int m, const u64* gtab, u32 tab_bytes,
                              cudaStream_t st);
@@ -98,6 +99,11 @@ cudaError_t launch_solve(const FieldParams& fp, const u64* a, size_t n, const u6
 // sizes validated by the caller.
 cudaError_t launch_convolve(const FieldParams& fp, const u64* a, size_t m, const u64* b, size_t n, size_t lo, size_t count,
                             u64* c, cudaStream_t st);
+
+// K11 (inst_select.cu): out[h] = (mask[h] != 0) != invert ? X(h) : Y(h), a side being x[h] * xs + xt, or the constant xt
+// when x is null (xs, xt: L canonical limbs each).  Prime fields; sizes validated by the caller.
+cudaError_t launch_select(const FieldParams& fp, const unsigned char* mask, bool invert, const u64* x, const u64* xs,
+                          const u64* xt, const u64* y, const u64* ys, const u64* yt, u64* out, size_t n, cudaStream_t st);
 
 extern template struct Launch<1>;
 extern template struct Launch<2>;

@@ -95,7 +95,7 @@ int mpyc_sm_count();
 
 template <int L>
 cudaError_t Launch<L>::inv_batch(const FieldParams& fp, const ExpParams& ex, const u64* a, u64* out, int* zero_flag,
-                                 size_t n, cudaStream_t st) {
+                                 size_t n, cudaStream_t st, const u64* num) {
     // batch length: as long as possible while every SM still gets >= 1024 threads; <= 32
     int B = 1;
     const size_t per_wave = (size_t)mpyc_sm_count() * 1024;
@@ -105,7 +105,9 @@ cudaError_t Launch<L>::inv_batch(const FieldParams& fp, const ExpParams& ex, con
         if (v >= 1 && v <= 1024) B = v;
     }
     const size_t T = (n + B - 1) / B;
-#define M(K) return launch_kernel(k_inv_batch<L, K>, T, 0, st, fp, ex, a, out, zero_flag, n, T, B)
+#define M(K)                                                                                                      \
+    if (num) return launch_kernel(k_inv_batch<L, K, true>, T, 0, st, fp, ex, a, out, zero_flag, n, T, B, num);     \
+    return launch_kernel(k_inv_batch<L, K, false>, T, 0, st, fp, ex, a, out, zero_flag, n, T, B, (const u64*)nullptr)
     KIND_SWITCH(fp.kind, M)
 #undef M
     return cudaErrorInvalidValue;

@@ -583,6 +583,75 @@ def convolve(ctx, a: DeviceArray, m, b: DeviceArray, n, lo, count):
     return out
 
 
+# ---- K11: division and selection (k_inv_batch with a numerator, csrc/select.cuh) ------------------------------------
+
+def divide(num: DeviceArray, den: DeviceArray):
+    """num[h] * den[h]^-1 in one Montgomery-trick pass (FiniteFieldArray.__truediv__, mpyc/finfields.py:1199-1206);
+    ZeroDivisionError if any den[h] == 0."""
+    if num.ctx is not den.ctx or num.n != den.n:
+        raise ValueError('divide: operands must share field and length')
+    num._check_contiguous()
+    den._check_contiguous()
+    out = num._like()
+    check(lib.mpyc_b200_ff_div(num.ctx.handle, num.ptr, den.ptr, out.ptr, num.n, _stream_ptr()))
+    return out
+
+
+def _mask_tensor(mask, n, where):
+    """A device uint8 tensor of n bytes from a device tensor (any dtype, nonzero = true) or a host bool / integer array."""
+    if isinstance(mask, torch.Tensor):
+        if mask.dtype not in (torch.uint8, torch.bool):
+            mask = mask != 0
+        mask = mask.reshape(-1).to(device=where, dtype=torch.uint8).contiguous()
+    else:
+        a = np.asarray(mask)
+        if a.dtype.kind not in 'biu':
+            raise TypeError('select: the mask must be a bool or integer array')
+        mask = torch.from_numpy(np.ascontiguousarray(a.reshape(-1) != 0).view(np.uint8)).to(where)
+    if mask.numel() != n:
+        raise ValueError(f'select: the mask holds {mask.numel()} entries, not {n}')
+    return mask
+
+
+def select(mask, x, x_map, y, y_map, n=None, invert=False):
+    """out[h] = mask[h] ? x[h] * sx + tx : y[h] * sy + ty (with invert: the other side), the np.where of field arrays and
+    raw share values (mpyc/runtime.py:1819, 3614-3615).  x, y: DeviceArrays, or None for the constant tx / ty;
+    x_map = (sx, tx), y_map = (sy, ty): public integers, reduced here.  mask: a device tensor or a host bool / integer
+    array (uploaded).  n: the element count (needed when both sides are constants)."""
+    arrays = [a for a in (x, y) if a is not None]
+    if not arrays:
+        raise ValueError('select: at least one side must be an array')
+    ctx = arrays[0].ctx
+    if n is None:
+        n = arrays[0].n
+    for a in arrays:
+        if a.ctx is not ctx or a.n != n:
+            raise ValueError('select: arrays must share field and length')
+        a._check_contiguous()
+    where = arrays[0].t.device
+    m = _mask_tensor(mask, n, where)
+    q, L = ctx.order, ctx.nlimbs
+
+    def st(sm):
+        s, t = sm
+        return _cabi.u64_array(_cabi.int_to_limbs(int(s) % q, L) + _cabi.int_to_limbs(int(t) % q, L))
+    out = DeviceArray.empty(ctx, n, where)
+    null = ctypes.c_void_p(0)
+    check(lib.mpyc_b200_ff_select(ctx.handle, ctypes.c_void_p(m.data_ptr()), 1 if invert else 0, x.ptr if x is not None else null,
+                                  st(x_map), y.ptr if y is not None else null, st(y_map), out.ptr, n, _stream_ptr()))
+    return out
+
+
+def nonzero_mask(a: DeviceArray):
+    """a != 0 as a device uint8 tensor (k_nonzero), without reading the count back to the host."""
+    a._check_contiguous()
+    mask = torch.empty(a.n, dtype=torch.uint8, device=a.t.device)
+    cnt = torch.zeros(1, dtype=torch.int64, device=a.t.device)
+    check(lib.mpyc_b200_ff_nonzero(a.ctx.handle, a.ptr, ctypes.c_void_p(mask.data_ptr()), ctypes.c_void_p(cnt.data_ptr()), a.n,
+                                   _stream_ptr()))
+    return mask
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

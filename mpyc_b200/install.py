@@ -116,13 +116,16 @@ def _install_operators(finfields_module, min_size):
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
     np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays.  Views, writes,
     axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
-    np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10; everything else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
+    np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10.  / (reflected and in place),
+    reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b; everything
+    else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
     from mpyc_b200 import _cabi, resident
     resident.min_size = int(min_size)
     cls = finfields_module.FiniteFieldArray
     names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
              '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
-             'sum', '__setitem__', 'transpose', 'swapaxes')
+             'sum', '__setitem__', 'transpose', 'swapaxes', '__truediv__', '__rtruediv__', '__itruediv__', 'reciprocal',
+             '__pow__', '__ipow__', 'sqrt', 'is_sqr')
     orig = {name: cls.__dict__[name] for name in names}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
@@ -216,6 +219,14 @@ def _install_operators(finfields_module, min_size):
             r = resident.convolve(type(self), args, kwargs)
             if r is not MISS:
                 return r
+        if func is np.where:
+            # a field element that comes first in np.where's arguments hands the call over with self the element
+            # (FiniteFieldElement.__array_function__, finfields.py:83-85)
+            klass = type(self) if isinstance(self, cls) else getattr(type(self), 'array', None)
+            if isinstance(klass, type) and issubclass(klass, cls):
+                r = resident.where(klass, args, kwargs)
+                if r is not MISS:
+                    return r
         return orig['__array_function__'](self, func, types, args, kwargs)
 
     def sum(self, *args, **kwargs):
@@ -231,6 +242,50 @@ def _install_operators(finfields_module, min_size):
         r = resident.equals(self, other, True)
         return orig['__ne__'](self, other) if r is MISS else r
 
+    def make_inplace(name, fn):
+        # `/=` and `**=` give self a new store, as `<<=` does: arrays sharing the old one keep their values
+        def method(self, other):
+            r = fn(self, other)
+            if r is MISS:
+                return orig[name](self, other)
+            slot_set(self, resident.raw_value(r))
+            return self
+        method.__name__ = name
+        method.__doc__ = orig[name].__doc__
+        return method
+
+    def __truediv__(self, other):
+        r = resident.divide(self, other)
+        return orig['__truediv__'](self, other) if r is MISS else r
+
+    def __rtruediv__(self, other):
+        r = resident.divide(self, other, reflected=True)
+        return orig['__rtruediv__'](self, other) if r is MISS else r
+
+    def reciprocal(self):
+        r = resident.reciprocal(self)
+        return orig['reciprocal'](self) if r is MISS else r
+
+    def __pow__(self, other):
+        r = resident.power(self, other)
+        return orig['__pow__'](self, other) if r is MISS else r
+
+    def sqrt(self, INV=False):
+        r = resident.sqrt(self, INV)
+        return orig['sqrt'](self, INV=INV) if r is MISS else r
+
+    def is_sqr(self):
+        r = resident.is_sqr(self)
+        return orig['is_sqr'](self) if r is MISS else r
+
+    cls.__truediv__ = __truediv__
+    cls.__rtruediv__ = __rtruediv__
+    cls.__itruediv__ = make_inplace('__itruediv__', resident.divide)
+    cls.reciprocal = reciprocal
+    cls.__pow__ = __pow__
+    cls.__ipow__ = make_inplace('__ipow__', resident.power)
+    cls.sqrt = sqrt
+    cls.is_sqr = is_sqr
     cls.__eq__ = __eq__
     cls.__ne__ = __ne__
     cls.__hash__ = orig_hash

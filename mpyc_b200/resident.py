@@ -28,7 +28,10 @@ This module lets the SAME objects carry their elements as limb buffers instead:
     4243-4273, 4413-4433).  Their `.value` reads get a ModValue, which evaluates those NumPy expressions mod p on the
     K1 / K6 kernels (csrc/local.cuh) instead of settling; see the class docstring for why that is exact.  The hooks
     around them (<< >>, contiguous __getitem__, np.concatenate(axis=0), == / != with a scalar, matrix/vector row
-    broadcast) keep np_prod's halving loop and np_is_zero_public limb-backed as well.
+    broadcast) keep np_prod's halving loop and np_is_zero_public limb-backed as well.  Runtime.np_reciprocal / np_lsb /
+    _np_is_zero / np_from_bits get ModValues too: `== 0`, np.count_nonzero and np.where (k_select) run on the limbs.
+  * Division, reciprocal, ** by an int, sqrt (Blum primes), is_sqr and np.where of field arrays run on K11 / K1b
+    (`divide`, `reciprocal`, `power`, `sqrt`, `is_sqr`, `where` below).
 
 All arithmetic runs on the GPU through the C ABI (`backend` below); there is no CPU path.  tests/oracle_device.py
 replaces `backend` by the oracle to exercise this module's host logic where no GPU exists.
@@ -123,11 +126,11 @@ class CudaBackend:
         dev, _ = self._dev()
         return dev.low_bits(self.to_store(ctx, a), nbits)
 
-    def nonzero(self, ctx, a):
-        """(bool ndarray a != 0, count)"""
+    def nonzero(self, ctx, a, want_mask=True):
+        """(bool ndarray a != 0, count); want_mask=False: (None, count), nothing but the count crosses to the host"""
         dev, _ = self._dev()
-        mask, count = dev.nonzero(self.to_store(ctx, a))
-        return mask.cpu().numpy(), count
+        mask, count = dev.nonzero(self.to_store(ctx, a), want_mask)
+        return (mask.cpu().numpy() if want_mask else None), count
 
     def bits_compose(self, ctx, bits, n, f, descending):
         dev, _ = self._dev()
@@ -197,6 +200,34 @@ class CudaBackend:
         """store of full[lo : lo + count] of the convolution of a (m) and b (n) (K10)"""
         dev, _ = self._dev()
         return dev.convolve(ctx, self.to_store(ctx, a), m, self.to_store(ctx, b), n, lo, count)
+
+    # ---- K11 and K1b, used by the division / selection hooks and ModValue ----
+    def divide(self, ctx, num, den):
+        """store of num / den elementwise (ZeroDivisionError for a zero in den)"""
+        dev, _ = self._dev()
+        return dev.divide(self.to_store(ctx, num), self.to_store(ctx, den))
+
+    def inverse(self, ctx, a):
+        return self.to_store(ctx, a).reciprocal()
+
+    def power(self, ctx, a, e):
+        """store of a ** e for a Python int e (negative: of the inverse; ZeroDivisionError for a zero then)"""
+        return self.to_store(ctx, a) ** e
+
+    def is_sqr(self, ctx, a):
+        """bool ndarray: a is a square (0 counts as one), K1b"""
+        return self.to_store(ctx, a).is_sqr().cpu().numpy()
+
+    def select(self, ctx, mask, x, x_map, y, y_map, n):
+        """store of mask ? x * sx + tx : y * sy + ty (x_map = (sx, tx), y_map = (sy, ty); a side None: its constant t).
+        mask: a host bool ndarray of n entries (uploaded), or a store whose nonzero elements select x -- that mask is built
+        by k_nonzero on the device and never crosses to the host."""
+        dev, _ = self._dev()
+        if not (isinstance(mask, np.ndarray) and mask.dtype == bool):
+            mask = dev.nonzero_mask(self.to_store(ctx, mask))
+        x = None if x is None else self.to_store(ctx, x)
+        y = None if y is None else self.to_store(ctx, y)
+        return dev.select(mask, x, x_map, y, y_map, n)
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -682,6 +713,10 @@ class ModValue:
         return self._materialise() != other
 
     def __eq__(self, other):
+        if self.store is not None and self._scalar(other) == 0:
+            self._need_exact('== 0')                               # `c.value == 0` (runtime.py:3614)
+            mask, _ = backend.nonzero(self.ctx, self.store)
+            return ~np.asarray(mask, dtype=bool).reshape(self.shape)
         if self.store is not None:
             self._need_exact('comparison')
         return self._materialise() == other
@@ -723,7 +758,95 @@ class ModValue:
               and len(self.shape) == 2 and self.size):
             calls['limb_ops'] += 1
             return self._new(backend.cumsum_rows(self.ctx, self._flush(), self.shape[0], self.shape[1]))
+        elif func is np.count_nonzero and len(args) == 1 and args[0] is self and not kwargs and self.store is not None:
+            self._need_exact('np.count_nonzero')                   # `np.count_nonzero(ar.value)` (runtime.py:1282)
+            calls['limb_ops'] += 1
+            return _count_nonzero(self.ctx, self.store)
+        elif func is np.where and len(args) == 3 and not kwargs:
+            r = _where(self.ctx, None, *args)
+            if r is not None:
+                return r
         return func(*_settled(args), **_settled(kwargs))
+
+
+def _count_nonzero(ctx, store):
+    """The number of nonzero elements of a store (k_nonzero; only the count crosses when the backend has K11)."""
+    if _divsel_backend():
+        return backend.nonzero(ctx, store, want_mask=False)[1]
+    return int(backend.nonzero(ctx, store)[1])
+
+
+def _array_class(x):
+    """type(x) when x is an array of a patched FiniteFieldArray class, else None."""
+    return type(x) if _slot is not None and isinstance(x, _slot.__objclass__) else None
+
+
+def _where_side(ctx, cls, x, shape):
+    """(store or None, s, t) for one side of np.where: the side's value is store * s + t, or the constant t when store is
+    None.  x: a ModValue (its pending affine map is passed on), a limb-backed value, an array of cls (limb-backed, or of
+    Python ints when it has at least min_size elements), an int or a field element of cls (reduced mod p, as the
+    reference's cls(.) does).  None for anything else."""
+    p = ctx.modulus
+    if type(x) is ModValue:
+        if x.store is None or x.ctx is not ctx or x.shape != shape:
+            return None
+        if x._sq:
+            x._flush()
+        return x.store, x._s, x._t
+    if type(x) is LimbValue:
+        return (x.store, 1, 0) if x.store is not None and x.ctx is ctx and x.shape == shape else None
+    xc = _array_class(x)
+    if xc is not None:
+        if cls is None:
+            cls = xc
+        if xc is not cls or _ctx_of(xc) is not ctx:
+            return None
+        lv = as_limb_value(raw_value(x))
+        if lv is not None:
+            return (lv.store, 1, 0) if lv.shape == shape else None
+        if np.shape(raw_value(x)) != shape:
+            return None
+        op = _operand(ctx, cls, x)
+        return None if op is None else (op[0], 1, 0)
+    if cls is not None and isinstance(x, cls.field):
+        x = x.value
+    if type(x) is int:
+        return None, 1, x % p
+    return None
+
+
+def _where(ctx, cls, cond, x, y):
+    """np.where(cond, x, y) on k_select for a condition of the result's shape -- a host bool / integer ndarray, or an exact
+    ModValue / limb-backed LimbValue whose != 0 mask k_nonzero builds on the device -- and sides of _where_side, at least
+    one of them an array.  The result is what the reference returns: an array of the sides' FiniteFieldArray class when
+    one side is such an array (FiniteFieldArray.__array_function__ wraps np.where's result, finfields.py:801-807), else a
+    (non-exact) ModValue for the object ndarray np.where makes of raw values.  None leaves the call to NumPy on the
+    settled values (and always without K11)."""
+    if not _divsel_backend() or ctx.binary:
+        return None
+    if type(cond) is ModValue or type(cond) is LimbValue:
+        if cond.store is None or cond.ctx is not ctx:
+            return None
+        if type(cond) is ModValue:
+            cond._need_exact('np.where condition')
+        shape, mask = cond.shape, cond.store
+    elif type(cond) is np.ndarray and cond.dtype.kind in 'biu':
+        shape, mask = cond.shape, (cond != 0).reshape(-1)
+    else:
+        return None
+    n = layout._prod(shape)
+    if n == 0:
+        return None
+    sides = [_where_side(ctx, cls, v, shape) for v in (x, y)]
+    if any(sd is None for sd in sides) or all(sd[0] is None for sd in sides):
+        return None
+    calls['limb_ops'] += 1
+    (xs, sx, tx), (ys, sy, ty) = sides
+    store = backend.select(ctx, mask, xs, (sx, tx), ys, (sy, ty), n)
+    out_cls = cls or _array_class(x) or _array_class(y)
+    if out_cls is not None:
+        return _wrap(out_cls, ctx, store, shape)
+    return ModValue(ctx, store, shape)
 
 
 def _settled(x):
@@ -902,6 +1025,10 @@ _MOD_SOURCES = {
     'np_trunc': 'e6354dbb71d6369d8bef9b065bef0cb65b1dc55631634954792f7945e087e3ad',           # runtime.py:838-872
     'np_sgn': '936eb16da844a41f636537f44306b80fff9aea3834ba205e187e6ba5a24547ad',             # runtime.py:3622-3694
     'np_to_bits': 'fb87bacf263e7c49f50422bba78d6bbf24fb200bc068983a511619da6bd16c1a',         # runtime.py:4391-4441
+    'np_reciprocal': '0ebb2c0f58c50e5229f2586b7f2db9e3ca18a1bed3486c7f28aa047095af0c00',      # runtime.py:1250-1294
+    'np_lsb': '4307852ce433d97be6c3bd63dbcc6a9c644b6acfd986a7fbbbac3eaa90c31bfb',             # runtime.py:1800-1822
+    '_np_is_zero': 'd2beb72e8b098a8e79dbdd2438f24e0972b9a6c46073fbad7a13bec0a6c761f0',        # runtime.py:3581-3620
+    'np_from_bits': '64d71aeb3dbed028a8046d6176b2fd8c8b38661bcd831ee069d3d1749338956c',       # runtime.py:4475-4484
 }
 
 
@@ -1683,6 +1810,176 @@ def convolve(cls, args, kwargs):
     s, g = min(m, n), max(m, n)
     lo, count = {'full': (0, m + n - 1), 'same': ((s - 1) // 2, g), 'valid': (s - 1, g - s + 1)}[mode]
     return _wrap(cls, ctx, backend.convolve(ctx, stores[0], m, stores[1], n, lo, count), (count,))
+
+
+# ---- K11: division, powers, square roots and np.where of field arrays ------------------------------------------------
+
+def _divsel_backend():
+    """K11's hooks run only when the backend has divide and select.  CudaBackend always does; a substituted backend without
+    them (a test stand-in) leaves division and selection to the reference's code, as before K11 existed."""
+    return hasattr(backend, 'divide') and hasattr(backend, 'select')
+
+
+def _unary_operand(a):
+    """(cls, ctx, store, shape) of a prime-field array that is limb-backed or an object array of at least min_size elements
+    (the rule of binop), not empty; None otherwise, and always without K11."""
+    cls = type(a)
+    ctx = _ctx_of(cls)
+    if ctx is None or ctx.binary or not _divsel_backend():
+        return None
+    mine = raw_value(a)
+    if as_limb_value(mine) is None and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
+        return None
+    op = _operand(ctx, cls, a)
+    if op is None or not layout._prod(op[1]):
+        return None
+    return (cls, ctx) + op
+
+
+def _public_scalar(cls, x):
+    """x as a Python int when it is an int (not a bool) or an element of cls.field -- what the reference's _coerce passes
+    on for a scalar; None otherwise."""
+    if isinstance(x, cls.field):
+        x = x.value
+    return x if isinstance(x, int) and not isinstance(x, bool) else None
+
+
+def _zero(cls):
+    z = np.empty(1, dtype=object)
+    z[0] = 0
+    return z
+
+
+def _reference_error(fn):
+    """Raise what the reference raises for a zero where an inverse is needed: fn runs the reference's own code on a single
+    zero (its message depends on whether gmpy2 is installed).  Falls back to ZeroDivisionError if it does not raise."""
+    fn()
+    raise ZeroDivisionError('invert() no inverse exists')
+
+
+def divide(self, other, reflected=False):
+    """self / other (reflected: other / self) for a limb-backed or large prime-field array (FiniteFieldArray.__truediv__ /
+    __rtruediv__, finfields.py:1199-1215): by a same-shape array of the class in one ff_div pass; by an int or field element
+    as a product with its inverse, computed on the host; an int or field element divided by the array as ff_inv and a
+    scalar product.  A zero divisor raises the reference's exception.  Returns a limb-backed array, or _MISS (broadcasting,
+    other operand types, binary fields, backends without K11)."""
+    cls = type(self)
+    ctx = _ctx_of(cls)
+    if ctx is None or ctx.binary or not _divsel_backend():
+        return _MISS
+    k = _public_scalar(cls, other)
+    if k is None and not reflected and type(other) is cls:
+        mine, theirs = raw_value(self), raw_value(other)
+        limbish = as_limb_value(mine) is not None or as_limb_value(theirs) is not None
+        if not limbish and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
+            return _MISS
+        if np.shape(mine) != np.shape(theirs) or not layout._prod(np.shape(mine)):
+            return _MISS
+        a, b = _operand(ctx, cls, self), _operand(ctx, cls, other)
+        if a is None or b is None:
+            return _MISS
+        try:
+            out = backend.divide(ctx, a[0], b[0])
+        except ZeroDivisionError:
+            _reference_error(lambda: cls._reciprocal(_zero(cls)))
+        return _wrap(cls, ctx, out, a[1])
+    if k is None:
+        return _MISS
+    op = _unary_operand(self)
+    if op is None:
+        return _MISS
+    _, _, store, shape = op
+    p = ctx.modulus
+    if not reflected:
+        if k % p == 0:
+            _reference_error(lambda: cls._reciprocal(0))
+        return _wrap(cls, ctx, backend.binop_scalar(ctx, _cabi.OP_MUL, store, pow(k, -1, p)), shape)
+    try:
+        inv = backend.inverse(ctx, store)
+    except ZeroDivisionError:
+        _reference_error(lambda: cls._reciprocal(_zero(cls)))
+    calls['limb_ops'] += 1
+    return _wrap(cls, ctx, backend.binop_scalar(ctx, _cabi.OP_MUL, inv, k % p), shape)
+
+
+def reciprocal(self):
+    """self.reciprocal() (finfields.py:1278-1281) on ff_inv: a limb-backed array, or _MISS as for divide."""
+    op = _unary_operand(self)
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    try:
+        out = backend.inverse(ctx, store)
+    except ZeroDivisionError:
+        _reference_error(lambda: cls._reciprocal(_zero(cls)))
+    return _wrap(cls, ctx, out, shape)
+
+
+def power(self, e):
+    """self ** e for a Python int e (finfields.py:1159-1167,1408-1414; powmod semantics: a negative e inverts first, e == 0
+    gives ones, 0 ** 0 included).  A zero with e < 0 raises the reference's exception.  _MISS for other exponents (ndarray,
+    NumPy or bool ones) and as for divide."""
+    if type(e) is not int:
+        return _MISS
+    op = _unary_operand(self)
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    if e == 0:
+        return _wrap(cls, ctx, backend.axpb(ctx, store, 0, 1), shape)
+    try:
+        out = backend.power(ctx, store, e)
+    except ZeroDivisionError:
+        _reference_error(lambda: cls._pow(_zero(cls), e))
+    return _wrap(cls, ctx, out, shape)
+
+
+def sqrt(self, INV=False):
+    """self.sqrt(INV) for Blum primes (PrimeFieldArray._sqrt, finfields.py:1424-1438) on K1b; INV with a zero raises the
+    reference's ZeroDivisionError('no inverse sqrt of 0').  _MISS for other primes and as for divide."""
+    op = _unary_operand(self)
+    if op is None or not isinstance(INV, bool):
+        return _MISS
+    cls, ctx, store, shape = op
+    if ctx.modulus & 3 != 3:
+        return _MISS
+    try:
+        out = backend.sqrt(ctx, store, INV)
+    except ZeroDivisionError:
+        _reference_error(lambda: cls._sqrt(_zero(cls), INV=True))
+    return _wrap(cls, ctx, out, shape)
+
+
+def is_sqr(self):
+    """self.is_sqr() (finfields.py:1298-1300, 1463-1470) on K1b: a host bool ndarray of the array's shape (0 counts as a
+    square).  _MISS for 0-d arrays and as for divide."""
+    op = _unary_operand(self)
+    if op is None or not op[3]:
+        return _MISS
+    cls, ctx, store, shape = op
+    calls['limb_ops'] += 1
+    return np.asarray(backend.is_sqr(ctx, store), dtype=bool).reshape(shape)
+
+
+def where(cls, args, kwargs):
+    """np.where(cond, x, y) with field arrays (FiniteFieldArray.__array_function__, finfields.py:766-819) on k_select: cond a
+    bool or integer ndarray of the result's shape, x and y arrays of cls of that shape, ints or field elements of cls, at
+    least one an array.  A limb-backed array of cls, or _MISS -- so that the reference keeps its own results and errors --
+    for binary fields, broadcasting, the one-argument form, keywords, other operand types and backends without K11."""
+    ctx = _ctx_of(cls)
+    if len(args) != 3 or kwargs or ctx is None or ctx.binary:
+        return _MISS
+    cond, x, y = args
+    if type(cond) is not np.ndarray:
+        return _MISS
+    arrays = [v for v in (x, y) if type(v) is cls]
+    if not arrays:
+        return _MISS
+    vals = [raw_value(v) for v in arrays]
+    if all(as_limb_value(v) is None for v in vals) and not any(isinstance(v, np.ndarray) and v.size >= min_size for v in vals):
+        return _MISS
+    r = _where(ctx, cls, cond, x, y)
+    return _MISS if r is None else r
 
 
 def conv2d(x, W, b):
