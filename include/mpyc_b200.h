@@ -233,6 +233,20 @@ int mpyc_b200_ff_div(const mpyc_b200_field* f, const void* d_num, const void* d_
 int mpyc_b200_ff_select(const mpyc_b200_field* f, const uint8_t* d_mask, int invert, const void* d_x, const uint64_t* h_x_st,
                         const void* d_y, const uint64_t* h_y_st, void* d_out, size_t n, void* stream);
 
+/* ---- per-element exponents (K12) ----------------------------------------------------------------
+ * d_out[h] = base(h)^e[h] mod p (PrimeFieldArray._pow with an exponent array, finfields.py:1409-1414; gmpy.powmod_exp_list,
+ * gmpy.py:288-290, which Runtime._np_pow_public_int_base_secret_integral_exponent calls twice, runtime.py:1408,1422).
+ * d_exps: n exponents of exp_limbs (1..4) little-endian 64-bit limbs each, none wider than exp_bits <= 64 * exp_limbs bits
+ * (the loop bound); not reduced.  Exactly one base:
+ *   h_base (L canonical limbs on the host): a public base for every element (fixed-base comb).  d_signs (n bytes, may be
+ *     null): a nonzero byte makes that exponent negative, base^-e[h]; MPYC_B200_EZERODIV for a zero base with d_signs.
+ *   d_base (n elements): one base per element; exponents are non-negative (d_signs must be null).
+ * Buffers need 8-byte alignment only.  Prime fields (MPYC_B200_EUNSUPPORTED otherwise); MPYC_B200_EINVAL before any CUDA
+ * call for null buffers, both or neither base, d_signs with d_base, a non-canonical h_base, exp_limbs outside 1..4,
+ * exp_bits > 64 * exp_limbs, byte counts that overflow and an output that overlaps an input. */
+int mpyc_b200_ff_pow_exp(const mpyc_b200_field* f, const void* d_base, const uint64_t* h_base, const uint64_t* d_exps,
+                         int exp_limbs, int exp_bits, const uint8_t* d_signs, size_t n, void* d_out, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -60,3 +60,35 @@ def limbs_to_wire(limbs, ctx):
     n = limbs.shape[0]
     raw = np.ascontiguousarray(limbs, dtype='<u8').view(np.uint8).reshape(n, 8 * ctx.nlimbs)
     return np.ascontiguousarray(raw[:, :r]).tobytes()
+
+
+MAX_EXP_LIMBS = 4     # K12 takes exponents of up to 256 bits
+
+
+def exponents_to_limbs(e):
+    """Exponents for K12 (mpyc_b200_ff_pow_exp): an int64 / uint64 ndarray, an object ndarray of Python ints, or a list /
+    tuple of Python ints -> (limbs uint64 (n, EL), signs uint8 (n,) or None when no entry is negative, B), with EL =
+    max(1, ceil(B / 64)) limbs of each magnitude and B the largest bit length.  None when not covered: other dtypes (bool,
+    float, smaller integers), entries that are not ints, or exponents wider than 256 bits."""
+    if isinstance(e, np.ndarray) and e.dtype.kind in 'iu':
+        if e.dtype.itemsize != 8:
+            return None
+        u = np.ascontiguousarray(e.reshape(-1)).view(np.uint64)
+        signs = None
+        if e.dtype.kind == 'i' and (neg := u >> np.uint64(63)).any():
+            signs = neg.astype(np.uint8)
+            u = np.where(signs != 0, ~u + np.uint64(1), u)      # |e|, also for -2^63
+        top = int(u.max()) if u.size else 0
+        return u.reshape(-1, 1), signs, top.bit_length()
+    if isinstance(e, np.ndarray):
+        if e.dtype != object:
+            return None
+        e = e.reshape(-1).tolist()
+    elif not isinstance(e, (list, tuple)):
+        return None
+    r = _pycodec.pack_exponents(e, MAX_EXP_LIMBS)
+    if r is None:
+        return None
+    limbs, signs, bits, el = r
+    signs = None if signs is None else np.frombuffer(signs, dtype=np.uint8)
+    return np.frombuffer(limbs, dtype='<u8').reshape(-1, el), signs, bits

@@ -993,6 +993,93 @@ MPYC_API int mpyc_b200_ff_select(const mpyc_b200_field* f, const uint8_t* d_mask
                          "ff_select launch");
 }
 
+// ---------------------------------------------------------------------------------------
+// K12: per-element exponents (powexp.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+// The comb window of the fixed-base form: the widest w <= 8 whose tables (one, or two with signs) fit MPYC_PE_SMEM_MAX.
+// An element costs ceil(B / w) - 1 products, the host ceil(B / w) 2^w to build a table.
+static int powexp_window(int bits, int L, int ntab, int* nwin, u32* bytes) {
+    for (int w = 8; w >= 1; w--) {
+        const int nw = (bits + w - 1) / w;
+        const size_t b = (size_t)ntab * ((size_t)nw << w) * L * sizeof(u64);
+        if (b <= MPYC_PE_SMEM_MAX) {
+            *nwin = nw;
+            *bytes = (u32)b;
+            return w;
+        }
+    }
+    return 0;   // unreachable: w = 1 needs 2 * 256 * 2 * 32 bytes at most
+}
+
+// g(s, j, d) = b_s^(d 2^(w j)) in the domain, b_0 = base, b_1 = base^-1 (ntab == 2); false when base == 0 and ntab == 2
+static bool powexp_tables(const FieldParams& fp, const u64* base, int w, int nwin, int ntab, std::vector<u64>& host) {
+    return with_field(fp, [&](auto Lc, auto Kc) {
+        constexpr int L = decltype(Lc)::value;
+        constexpr int K = decltype(Kc)::value;
+        typedef Fp<L, K> F;
+        constexpr int N = 2 * L;
+        const size_t D = (size_t)1 << w;
+        host.assign((size_t)ntab * nwin * D * L, 0);
+        for (int s = 0; s < ntab; s++) {
+            u32 b[N], g[N];
+            for (int i = 0; i < L; i++) set64(b, i, base[i]);
+            if (s == 1 && !h_inv<L, K>(b, b, fp)) return 0;
+            F::to_dom(g, b, fp);                                  // g = b^(2^(w j)) for the current j
+            for (int j = 0; j < nwin; j++) {
+                u64* row = &host[((size_t)s * nwin + j) * D * L];
+                u32 x[N];
+                F::dom_one(x, fp);
+                for (size_t d = 0; d < D; d++) {
+                    for (int i = 0; i < L; i++) row[d * L + i] = get64(x, i);
+                    F::dmul(x, x, g, fp);
+                }
+                copy_n<N>(g, x);                                  // g^(2^w)
+            }
+        }
+        return 1;
+    }) == 1;
+}
+
+MPYC_API int mpyc_b200_ff_pow_exp(const mpyc_b200_field* f, const void* d_base, const uint64_t* h_base, const uint64_t* d_exps,
+                                  int exp_limbs, int exp_bits, const uint8_t* d_signs, size_t n, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_pow_exp: field is null")) return rc;
+    if ((d_base == nullptr) == (h_base == nullptr)) return fail(MPYC_B200_EINVAL, "ff_pow_exp: give exactly one of the two bases");
+    if (exp_limbs < 1 || exp_limbs > 4) return fail(MPYC_B200_EINVAL, "ff_pow_exp: exp_limbs must be 1..4");
+    if (exp_bits < 0 || exp_bits > 64 * exp_limbs) return fail(MPYC_B200_EINVAL, "ff_pow_exp: exp_bits exceeds 64 * exp_limbs");
+    if (d_signs && d_base) return fail(MPYC_B200_EINVAL, "ff_pow_exp: signs need the fixed base");
+    if (h_base && !canonical(f, h_base)) return fail(MPYC_B200_EINVAL, "ff_pow_exp: the base must be a canonical residue");
+    const size_t L = f->fp.L;
+    size_t bytes = 0, ebytes = 0;
+    if (__builtin_mul_overflow(n, L * sizeof(u64), &bytes) || bytes > (size_t)INT64_MAX ||
+        __builtin_mul_overflow(n, (size_t)exp_limbs * sizeof(u64), &ebytes) || ebytes > (size_t)INT64_MAX)
+        return fail(MPYC_B200_EINVAL, "ff_pow_exp: size overflow");
+    if (n == 0) return MPYC_B200_OK;
+    if (!d_exps || !d_out) return fail(MPYC_B200_EINVAL, "ff_pow_exp: null buffer");
+    if (bytes_overlap(d_out, bytes, d_exps, ebytes) || (d_signs && bytes_overlap(d_out, bytes, d_signs, n)) ||
+        (d_base && bytes_overlap(d_out, bytes, d_base, bytes)))
+        return fail(MPYC_B200_EINVAL, "ff_pow_exp: out overlaps an operand");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d_base)
+        return launch_status(launch_powexp(f->fp, (const u64*)d_base, nullptr, 0, 0, 0, (const u64*)d_exps, exp_limbs, exp_bits,
+                                           nullptr, (u64*)d_out, n, st),
+                             "ff_pow_exp launch");
+    const int ntab = d_signs ? 2 : 1;
+    int nwin = 0;
+    u32 tab_bytes = 0;
+    const int w = powexp_window(std::max(exp_bits, 1), (int)L, ntab, &nwin, &tab_bytes);
+    std::vector<u64> host;
+    if (!powexp_tables(f->fp, (const u64*)h_base, w, nwin, ntab, host)) return fail(MPYC_B200_EZERODIV, "inverse of zero");
+    u64* tab = nullptr;
+    CU(cudaMallocAsync(&tab, tab_bytes, st));
+    cudaError_t e = cudaMemcpyAsync(tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);   // host vector goes out of scope
+    if (e == cudaSuccess)
+        e = launch_powexp(f->fp, nullptr, tab, tab_bytes, w, nwin, (const u64*)d_exps, exp_limbs, exp_bits, d_signs, (u64*)d_out, n, st);
+    cudaFreeAsync(tab, st);
+    return launch_status(e, "ff_pow_exp launch");
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

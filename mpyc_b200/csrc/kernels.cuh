@@ -17,6 +17,7 @@
 //   K7   k_sum_cols / k_sum_rows, k_scan_cols / k_scan_rows (reduce.cuh)   np.sum / np.cumsum along any axis
 //   K8   k_copy_gather, k_copy_permute, k_binop_view (layout.cuh)   strided views, joins, broadcast arithmetic
 //   K11  k_inv_batch<NUM> (ff_div), k_select (select.cuh)   division and np.where       finfields.py:1199-1225
+//   K12  k_powexp_fixed, k_powexp_elem (powexp.cuh)   per-element exponents   finfields.py:1409-1414, gmpy.py:288-290
 #pragma once
 #include "ff_arith.cuh"
 

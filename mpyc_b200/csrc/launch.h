@@ -105,6 +105,13 @@ cudaError_t launch_convolve(const FieldParams& fp, const u64* a, size_t m, const
 cudaError_t launch_select(const FieldParams& fp, const unsigned char* mask, bool invert, const u64* x, const u64* xs,
                           const u64* xt, const u64* y, const u64* ys, const u64* yt, u64* out, size_t n, cudaStream_t st);
 
+// K12 (inst_powexp.cu): out[h] = base(h)^e[h], e[h] = el little-endian limbs of at most ebits bits.  tab non-null: the
+// fixed-base form, tab = comb tables of tab_bytes (<= MPYC_PE_SMEM_MAX) in the domain, window w, nwin windows, sgn (may be
+// null) picking the second table; else the per-element form on a.  Prime fields; sizes validated by the caller.
+#define MPYC_PE_SMEM_MAX (96u * 1024u)
+cudaError_t launch_powexp(const FieldParams& fp, const u64* a, const u64* tab, u32 tab_bytes, int w, int nwin, const u64* e,
+                          int el, int ebits, const unsigned char* sgn, u64* out, size_t n, cudaStream_t st);
+
 extern template struct Launch<1>;
 extern template struct Launch<2>;
 extern template struct Launch<3>;

@@ -217,8 +217,73 @@ static PyObject* unpack(PyObject* self, PyObject* args) {
     return out;
 }
 
+/* pack_exponents(seq, max_limbs) -> (limbs, signs, bits, el) or None: the magnitudes of a sequence of Python ints (not
+ * bools) as el = max(1, ceil(bits / 64)) little-endian 64-bit limbs each, bits the largest bit length; signs a bytearray
+ * with 1 for each negative entry, or None when there is none.  None when an entry is not an int or bits > 64 * max_limbs:
+ * the exponents of K12 (mpyc_b200.codec.exponents_to_limbs) are not reduced, so nothing wider has a place to go. */
+static PyObject* pack_exponents(PyObject* self, PyObject* args) {
+    PyObject* seq;
+    int max_limbs;
+    if (!PyArg_ParseTuple(args, "Oi", &seq, &max_limbs)) return NULL;
+    if (max_limbs < 1 || max_limbs > MAX_LIMBS - 1) {
+        PyErr_SetString(PyExc_ValueError, "pack_exponents: max_limbs must be 1..4");
+        return NULL;
+    }
+    PyObject* fast = PySequence_Fast(seq, "pack_exponents: expected a sequence of ints");
+    if (!fast) return NULL;
+    const Py_ssize_t n = PySequence_Fast_GET_SIZE(fast);
+    PyObject** items = PySequence_Fast_ITEMS(fast);
+    size_t bits = 0;
+    int negative = 0;
+    for (Py_ssize_t i = 0; i < n; i++) {
+        PyObject* v = items[i];
+        if (!PyLong_Check(v) || PyBool_Check(v)) {
+            Py_DECREF(fast);
+            Py_RETURN_NONE;
+        }
+        const size_t b = _PyLong_NumBits(v);          /* of |v| */
+        if (b == (size_t)-1 && PyErr_Occurred()) goto fail0;
+        if (b > bits) bits = b;
+        if (_PyLong_Sign(v) < 0) negative = 1;
+    }
+    if (bits > (size_t)64 * max_limbs) {
+        Py_DECREF(fast);
+        Py_RETURN_NONE;
+    }
+    const Py_ssize_t el = bits ? (Py_ssize_t)((bits + 63) / 64) : 1;
+    PyObject* limbs = PyByteArray_FromStringAndSize(NULL, n * el * 8);
+    PyObject* signs = negative ? PyByteArray_FromStringAndSize(NULL, n) : (Py_INCREF(Py_None), Py_None);
+    if (!limbs || !signs) {
+        Py_XDECREF(limbs);
+        Py_XDECREF(signs);
+        goto fail0;
+    }
+    unsigned char* dst = (unsigned char*)PyByteArray_AS_STRING(limbs);
+    unsigned char* sg = negative ? (unsigned char*)PyByteArray_AS_STRING(signs) : NULL;
+    for (Py_ssize_t i = 0; i < n; i++) {
+        PyObject* v = items[i];
+        const int neg = _PyLong_Sign(v) < 0;
+        if (sg) sg[i] = (unsigned char)neg;
+        PyObject* owned = neg ? PyNumber_Negative(v) : NULL;
+        if (neg && !owned) goto fail;
+        const int rc = as_bytes(owned ? owned : v, dst + i * el * 8, (size_t)(el * 8));
+        Py_XDECREF(owned);
+        if (rc < 0) goto fail;
+    }
+    Py_DECREF(fast);
+    PyObject* r = Py_BuildValue("(NNnn)", limbs, signs, (Py_ssize_t)bits, el);
+    return r;
+fail:
+    Py_DECREF(limbs);
+    Py_DECREF(signs);
+fail0:
+    Py_DECREF(fast);
+    return NULL;
+}
+
 static PyMethodDef methods[] = {
     {"pack", pack, METH_VARARGS, "pack(seq, nbytes, modulus) -> bytearray (little-endian, reduced mod modulus)"},
+    {"pack_exponents", pack_exponents, METH_VARARGS, "pack_exponents(seq, max_limbs) -> (limbs, signs or None, bits, el) or None"},
     {"unpack", unpack, METH_VARARGS, "unpack(buffer, nbytes) -> list of ints"},
     {"unpack_into", unpack_into, METH_VARARGS, "unpack_into(buffer, nbytes, address of n object slots)"},
     {NULL, NULL, 0, NULL}};

@@ -652,6 +652,37 @@ def nonzero_mask(a: DeviceArray):
     return mask
 
 
+# ---- K12: per-element exponents (csrc/powexp.cuh) --------------------------------------------------------------------
+
+def pow_exp(ctx, base, exps, signs, bits, device=None):
+    """out[h] = base(h)^e[h] mod p (PrimeFieldArray._pow with an exponent array, mpyc/finfields.py:1409-1414;
+    gmpy.powmod_exp_list, mpyc/gmpy.py:288-290).  base: a DeviceArray (one base per element) or a Python int (one public
+    base, reduced here).  exps, signs, bits: codec.exponents_to_limbs's (limbs (n, EL), signs or None, B), uploaded here;
+    signs only with an int base.  ZeroDivisionError for a zero base with signs.  A DeviceArray of n elements."""
+    import torch
+    exps = np.ascontiguousarray(exps, dtype=np.uint64)
+    n, el = exps.shape
+    if isinstance(base, DeviceArray):
+        if base.ctx is not ctx or base.n != n:
+            raise ValueError('pow_exp: bases and exponents must share field and length')
+        base._check_contiguous()
+        where = base.t.device
+    else:
+        _require_cuda()
+        where = torch.device('cuda', torch.cuda.current_device()) if device is None else device
+    e = torch.from_numpy(exps.view(np.int64)).to(where)
+    s = torch.from_numpy(np.ascontiguousarray(signs, dtype=np.uint8)).to(where) if signs is not None else None
+    out = DeviceArray.empty(ctx, n, where)
+    null = ctypes.c_void_p(0)
+    if isinstance(base, DeviceArray):
+        d_base, h_base = base.ptr, null
+    else:
+        d_base, h_base = null, ctx.scalar_limbs(base)
+    check(lib.mpyc_b200_ff_pow_exp(ctx.handle, d_base, h_base, ctypes.c_void_p(e.data_ptr()), el, int(bits),
+                                   ctypes.c_void_p(s.data_ptr()) if s is not None else null, n, out.ptr, _stream_ptr(where)))
+    return out
+
+
 def binop_rows(a: DeviceArray, b: DeviceArray, op, rows, cols, reflected=False):
     """a (rows, cols) (op) b (cols) broadcast over the rows; reflected: b (op) a (mpyc/runtime.py:3670)."""
     if a.n != rows * cols or b.n != cols or a.ctx is not b.ctx:

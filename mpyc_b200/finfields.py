@@ -6,8 +6,9 @@ finfields.py:1408-1470) -- 5 us per element with the pure-Python stubs.  The fun
 signatures of those classmethods (value arrays in, value arrays out) and run one kernel over the whole
 array; mpyc_b200.install.install(finfields=...) assigns them over PrimeFieldArray's methods.
 
-Per-element exponents (a ** b with an array b) and non-Blum square roots are not batched here: those
-calls are handed back to the reference implementation that was in place before install().
+Per-element exponents (a ** b with an integer array b of a's shape, non-negative) run on K12 through the resident
+backend's pow_exp.  Other exponent arrays and non-Blum square roots are not batched here: those calls are handed back to
+the reference implementation that was in place before install().
 """
 import numpy as np
 
@@ -33,11 +34,32 @@ def reciprocal(cls, a):
     return _back(A.reciprocal(), shape)
 
 
+def _power_exp(cls, a, b):
+    """a ** b elementwise on K12 for an exponent ndarray b of a's shape (codec.exponents_to_limbs covers it, no entry
+    negative), through resident.backend.pow_exp; None when not covered or the backend has no pow_exp."""
+    from mpyc_b200 import resident
+    a = np.asarray(a, dtype=object)
+    if not resident._powexp_backend() or b.shape != a.shape or not a.size:
+        return None
+    ex = codec.exponents_to_limbs(b)
+    if ex is None or ex[1] is not None:
+        return None
+    ctx = context_for(cls.field.modulus)
+    resident.calls['pow_exp'] += 1
+    out = resident.backend.pow_exp(ctx, codec.ints_to_limbs(a.reshape(-1), ctx), ex[0], None, ex[2])
+    return codec.limbs_to_ints(resident.backend.to_host(ctx, out), ctx).reshape(a.shape)
+
+
 def power(cls, a, b, _fallback=None):
-    """PrimeFieldArray._pow (finfields.py:1408-1414) for one integer exponent (negative allowed)."""
+    """PrimeFieldArray._pow (finfields.py:1408-1414) for one integer exponent (negative allowed), or per element for an
+    integer exponent array of a's shape (K12)."""
     if isinstance(b, (int, np.integer)):
         ctx, shape, A = _to_device(cls, a)
         return _back(A ** int(b), shape)
+    if isinstance(b, np.ndarray):
+        r = _power_exp(cls, a, b)
+        if r is not None:
+            return r
     if _fallback is None:
         raise TypeError('per-element exponents are not batched by mpyc_b200')
     return _fallback(a, b)

@@ -109,6 +109,32 @@ def _install_finfields(finfields_module, min_size):
 
 _saved_ff = {}
 _saved_ops = {}
+_saved_gmpy = {}
+
+
+def _install_gmpy(thresha_module):
+    """mpyc.gmpy.powmod_exp_list -> K12 (mpyc_b200.resident.powmod_exp_list).  runtime.py imports the module as
+    `from mpyc import gmpy as gmpy2` and looks the function up at call time (runtime.py:24,1408,1422), so assigning over the
+    module attribute reaches Runtime._np_pow_public_int_base_secret_integral_exponent -- 2 ** x, np_pow with a public int
+    base and np_exp2 / np_exp -- with runtime.py unchanged.  Calls it does not cover go to the saved original."""
+    import importlib
+    from mpyc_b200 import resident
+    package = thresha_module.__name__.rpartition('.')[0]
+    try:
+        gmpy = importlib.import_module(package + '.gmpy') if package else None
+    except ImportError:
+        gmpy = None
+    if gmpy is None or not hasattr(gmpy, 'powmod_exp_list'):
+        return
+    theirs = gmpy.powmod_exp_list
+    _saved_gmpy.update({'module': gmpy, 'powmod_exp_list': theirs})
+
+    @functools.wraps(theirs)
+    def powmod_exp_list(base, exp_lst, mod, /):
+        r = resident.powmod_exp_list(base, exp_lst, mod)
+        return theirs(base, exp_lst, mod) if r is resident._MISS else r
+    powmod_exp_list.__mpyc_b200__ = True
+    gmpy.powmod_exp_list = powmod_exp_list
 
 
 def _install_operators(finfields_module, min_size):
@@ -117,7 +143,8 @@ def _install_operators(finfields_module, min_size):
     np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays.  Views, writes,
     axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
     np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10.  / (reflected and in place),
-    reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b; everything
+    reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b, and ** and **=
+    by an integer array of the same shape on K12; everything
     else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
     from mpyc_b200 import _cabi, resident
     resident.min_size = int(min_size)
@@ -324,6 +351,7 @@ def install(thresha_module=None, strict=False, device=0, finfields_module=None, 
     recombined / pseudorandom shares stay limb-backed in HBM between protocol steps; Python ints are created only
     where a value is actually looked at (input, output, raw-value arithmetic).  local_algebra (with resident): the raw-value
     arithmetic of Runtime.np_random_bits / np_trunc / np_sgn runs mod p on the device as well (resident.ModValue, K6 kernels).
+    resident=True also routes mpyc.gmpy.powmod_exp_list (2 ** x, np_pow, np_exp2, np_exp of secure arrays) to K12.
     Returns the list of patched names."""
     if thresha_module is None:
         import mpyc.thresha as thresha_module
@@ -351,6 +379,8 @@ def install(thresha_module=None, strict=False, device=0, finfields_module=None, 
             ours = getattr(engine, name)
         routed = min_size if name not in ('_recombination_vector', '_f_S_i') else 0
         setattr(thresha_module, name, _wrap(name, ours, theirs, strict, routed))
+    if resident:
+        _install_gmpy(thresha_module)
     return list(_NAMES)
 
 
@@ -367,6 +397,8 @@ def uninstall():
         for name, member in _saved_ops.items():
             setattr(cls, name, member)
         _saved_ops.clear()
+    if _saved_gmpy:
+        _saved_gmpy.pop('module').powmod_exp_list = _saved_gmpy.pop('powmod_exp_list')
     if _saved_ff:
         cls = _saved_ff.pop('cls')
         for name, member in _saved_ff.items():

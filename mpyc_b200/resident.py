@@ -46,7 +46,7 @@ import sys
 
 resident = False      # np_recombine / PRSS results stay limb-backed (set by install(resident=True))
 min_size = 1024       # plain object-array operands of fewer elements are left to the reference's operators
-calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0}    # counters (tests, profiling)
+calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0}    # counters (tests, profiling)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -228,6 +228,15 @@ class CudaBackend:
         x = None if x is None else self.to_store(ctx, x)
         y = None if y is None else self.to_store(ctx, y)
         return dev.select(mask, x, x_map, y, y_map, n)
+
+    # ---- K12, used by the per-element exponent hooks ----
+    def pow_exp(self, ctx, base, exps, signs, bits):
+        """store of base(h)^e[h]: base a store (one base per element, signs None) or a Python int (one public base);
+        exps, signs, bits as codec.exponents_to_limbs returns them (ZeroDivisionError for a zero int base with signs)"""
+        dev, where = self._dev()
+        if not isinstance(base, int):
+            base = self.to_store(ctx, base)
+        return dev.pow_exp(ctx, base, exps, signs, bits, device=where)
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -1917,8 +1926,10 @@ def reciprocal(self):
 
 def power(self, e):
     """self ** e for a Python int e (finfields.py:1159-1167,1408-1414; powmod semantics: a negative e inverts first, e == 0
-    gives ones, 0 ** 0 included).  A zero with e < 0 raises the reference's exception.  _MISS for other exponents (ndarray,
-    NumPy or bool ones) and as for divide."""
+    gives ones, 0 ** 0 included).  A zero with e < 0 raises the reference's exception.  An integer ndarray e of the array's
+    shape runs on K12 (`power_exp`).  _MISS for other exponents (NumPy or bool ones) and as for divide."""
+    if isinstance(e, np.ndarray):
+        return power_exp(self, e)
     if type(e) is not int:
         return _MISS
     op = _unary_operand(self)
@@ -1932,6 +1943,63 @@ def power(self, e):
     except ZeroDivisionError:
         _reference_error(lambda: cls._pow(_zero(cls), e))
     return _wrap(cls, ctx, out, shape)
+
+
+# ---- K12: per-element exponents ---------------------------------------------------------------------------------------
+
+def _powexp_backend():
+    """K12's hooks run only when the backend has pow_exp (CudaBackend does; a stand-in without it leaves these calls to the
+    reference's code)."""
+    return hasattr(backend, 'pow_exp')
+
+
+def _exponents(e, n):
+    """codec.exponents_to_limbs(e) for n exponents, or None (not covered, or another count)."""
+    r = codec.exponents_to_limbs(e)
+    return r if r is not None and r[0].shape[0] == n else None
+
+
+def power_exp(self, e):
+    """self ** e for an int64 / uint64 / object ndarray e of Python ints of exactly self's shape (finfields.py:1159-1167 with
+    PrimeFieldArray._pow, finfields.py:1409-1414), on k_powexp_elem.  _MISS -- the reference computes -- for broadcasting,
+    other dtypes, exponents wider than 256 bits, negative exponents, binary fields and backends without K12."""
+    if not _powexp_backend():
+        return _MISS
+    op = _unary_operand(self)
+    if op is None or e.shape != op[3]:
+        return _MISS
+    cls, ctx, store, shape = op
+    ex = _exponents(e, layout._prod(shape))
+    if ex is None or ex[1] is not None:
+        return _MISS
+    calls['pow_exp'] += 1
+    return _wrap(cls, ctx, backend.pow_exp(ctx, store, ex[0], None, ex[2]), shape)
+
+
+def powmod_exp_list(base, exp_lst, mod):
+    """gmpy.powmod_exp_list(base, exp_lst, mod) (mpyc/gmpy.py:288-290) on k_powexp_fixed: a list of Python ints base^y mod
+    mod for y in exp_lst.  Covered: mod the modulus of a prime field the engine already holds a context for, an int base,
+    and at least min_size exponents given as Python ints in a list / tuple or a 1-D object ndarray.  _MISS for everything
+    else -- NumPy integer exponents included: the reference's three-argument pow rejects them with a TypeError, which stays
+    its own -- and for a base = 0 (mod mod) with a negative exponent, so that the error is the reference's."""
+    if not _powexp_backend() or type(base) is not int or type(mod) is not int:
+        return _MISS
+    from mpyc_b200 import field
+    ctx = field._contexts.get((mod, False))
+    listed = isinstance(exp_lst, (list, tuple)) or (isinstance(exp_lst, np.ndarray) and exp_lst.dtype == object
+                                                     and exp_lst.ndim == 1)
+    if ctx is None or not listed or len(exp_lst) < max(min_size, 1):
+        return _MISS
+    ex = codec.exponents_to_limbs(exp_lst)
+    if ex is None:
+        return _MISS
+    limbs, signs, bits = ex
+    b = base % mod
+    if b == 0 and signs is not None:
+        return _MISS
+    calls['pow_exp'] += 1
+    out = backend.pow_exp(ctx, b, limbs, signs, bits)
+    return codec.limbs_to_ints(backend.to_host(ctx, out), ctx).tolist()
 
 
 def sqrt(self, INV=False):
