@@ -219,9 +219,10 @@ int mpyc_b200_ff_convolve(const mpyc_b200_field* f, const void* d_a, size_t m, c
 /* ---- division and selection (K11) ---------------------------------------------------------------
  * d_out[h] = d_num[h] * d_den[h]^-1 mod p in one Montgomery-trick pass (FiniteFieldArray.__truediv__ / __itruediv__,
  * finfields.py:1199-1225, whose `self.value * cls._reciprocal(other)` it replaces; Runtime.np_reciprocal's `r / ar`,
- * runtime.py:1290).  Prime fields.  MPYC_B200_EZERODIV if any d_den[h] == 0 (synchronises the stream, as ff_inv).
- * MPYC_B200_EINVAL before any CUDA call for null buffers, byte counts that overflow and an output that overlaps either
- * input (the forward pass keeps prefix products in d_out); num and den may be the same buffer. */
+ * runtime.py:1290).  Prime fields.  MPYC_B200_EZERODIV if any d_den[h] == 0 (synchronises the stream, as ff_inv); d_out
+ * then holds 0 where d_den[h] == 0 and the quotient everywhere else: a zero does not spoil its batch.  MPYC_B200_EINVAL
+ * before any CUDA call for null buffers, byte counts that overflow and an output that overlaps either input (the forward
+ * pass keeps prefix products in d_out); num and den may be the same buffer. */
 int mpyc_b200_ff_div(const mpyc_b200_field* f, const void* d_num, const void* d_den, void* d_out, size_t n, void* stream);
 
 /* d_out[h] = ((d_mask[h] != 0) != invert) ? X(h) : Y(h) mod p: np.where(cond, x, y) of field arrays and raw share values
