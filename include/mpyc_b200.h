@@ -248,6 +248,28 @@ int mpyc_b200_ff_select(const mpyc_b200_field* f, const uint8_t* d_mask, int inv
 int mpyc_b200_ff_pow_exp(const mpyc_b200_field* f, const void* d_base, const uint64_t* h_base, const uint64_t* d_exps,
                          int exp_limbs, int exp_bits, const uint8_t* d_signs, size_t n, void* d_out, void* stream);
 
+/* ---- products, running products and all / any along an axis (K13; prime fields) -----------------
+ * d_in is viewed as (outer, len, inner) as for K7.  Any 8-byte aligned buffers work (a slice may start at any element).
+ * MPYC_B200_EINVAL before any CUDA call for null buffers, byte counts that overflow, an output that overlaps the input and
+ * (prod) a non-canonical initial; MPYC_B200_EUNSUPPORTED for binary fields.
+ *
+ * np.prod(a, axis, initial=...) / FiniteFieldArray.prod (mpyc/finfields.py:1339-1349, 766-819): out[o][i] =
+ * initial * prod_r in[o][r][i] mod p, out (outer, inner).  initial: L canonical host limbs, or NULL for 1.  len == 0 writes
+ * initial. */
+int mpyc_b200_ff_prod_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                           const uint64_t* initial, void* d_out, void* stream);
+/* np.cumprod(a, axis) / np.cumulative_prod(a, axis, include_initial) (finfields.py:766-819): out[o][inc + r][i] =
+ * prod_{r' <= r} in[o][r'][i] mod p, out (outer, len + inc, inner) with inc = include_initial != 0 and a row of ones first
+ * when inc. */
+int mpyc_b200_ff_cumprod_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                              int include_initial, void* d_out, void* stream);
+/* np.all(a, axis) (any == 0) / np.any(a, axis) (any != 0) (finfields.py:766-819, whose `cls(bool_array)` this is;
+ * Runtime.np_is_zero_public's `np.all(...)`, runtime.py:965): out[o][i] = 1 if every (any) in[o][r][i] is nonzero, else 0,
+ * as canonical limbs, out (outer, inner).  len == 0 gives 1 (all) and 0 (any).  For a reduction over the whole array,
+ * mpyc_b200_ff_nonzero's count answers both. */
+int mpyc_b200_ff_all_any_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner, int any,
+                              void* d_out, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -1080,6 +1080,58 @@ MPYC_API int mpyc_b200_ff_pow_exp(const mpyc_b200_field* f, const void* d_base, 
     return launch_status(e, "ff_pow_exp launch");
 }
 
+// ---------------------------------------------------------------------------------------
+// K13: products, running products and all / any along an axis (prod.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+// byte counts of an (outer, len, inner) input and an (outer, out_len, inner) output; false when one overflows
+static bool axis_bytes(const mpyc_b200_field* f, size_t outer, size_t len, size_t out_len, size_t inner, size_t* in_b, size_t* out_b) {
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    return !__builtin_mul_overflow(outer, len, in_b) && !__builtin_mul_overflow(*in_b, inner, in_b) &&
+           !__builtin_mul_overflow(*in_b, E, in_b) && *in_b <= (size_t)INT64_MAX && !__builtin_mul_overflow(outer, out_len, out_b) &&
+           !__builtin_mul_overflow(*out_b, inner, out_b) && !__builtin_mul_overflow(*out_b, E, out_b) && *out_b <= (size_t)INT64_MAX;
+}
+
+MPYC_API int mpyc_b200_ff_prod_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                                    const uint64_t* initial, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_prod_axis: field is null")) return rc;
+    size_t ib = 0, ob = 0;
+    if (!axis_bytes(f, outer, len, 1, inner, &ib, &ob)) return fail(MPYC_B200_EINVAL, "ff_prod_axis: size overflow");
+    if (initial && !canonical(f, initial)) return fail(MPYC_B200_EINVAL, "ff_prod_axis: initial must be a canonical residue");
+    if (outer == 0 || inner == 0) return MPYC_B200_OK;
+    if (!d_out || (len && !d_in)) return fail(MPYC_B200_EINVAL, "ff_prod_axis: null buffer");
+    if (bytes_overlap(d_in, ib, d_out, ob)) return fail(MPYC_B200_EINVAL, "ff_prod_axis: out overlaps the input");
+    return launch_status(launch_prod_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, (const u64*)initial,
+                                          (cudaStream_t)stream),
+                         "ff_prod_axis launch");
+}
+
+MPYC_API int mpyc_b200_ff_cumprod_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner,
+                                       int include_initial, void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_cumprod_axis: field is null")) return rc;
+    const size_t inc = include_initial ? 1 : 0;
+    size_t ib = 0, ob = 0;
+    if (len > SIZE_MAX - inc || !axis_bytes(f, outer, len, len + inc, inner, &ib, &ob))
+        return fail(MPYC_B200_EINVAL, "ff_cumprod_axis: size overflow");
+    if (outer == 0 || inner == 0 || len + inc == 0) return MPYC_B200_OK;
+    if (!d_out || (len && !d_in)) return fail(MPYC_B200_EINVAL, "ff_cumprod_axis: null buffer");
+    if (bytes_overlap(d_in, ib, d_out, ob)) return fail(MPYC_B200_EINVAL, "ff_cumprod_axis: out overlaps the input");
+    return launch_status(launch_cumprod_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, inc != 0, (cudaStream_t)stream),
+                         "ff_cumprod_axis launch");
+}
+
+MPYC_API int mpyc_b200_ff_all_any_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner, int any,
+                                       void* d_out, void* stream) {
+    if (int rc = prime_only(f, "ff_all_any_axis: field is null")) return rc;
+    size_t ib = 0, ob = 0;
+    if (!axis_bytes(f, outer, len, 1, inner, &ib, &ob)) return fail(MPYC_B200_EINVAL, "ff_all_any_axis: size overflow");
+    if (outer == 0 || inner == 0) return MPYC_B200_OK;
+    if (!d_out || (len && !d_in)) return fail(MPYC_B200_EINVAL, "ff_all_any_axis: null buffer");
+    if (bytes_overlap(d_in, ib, d_out, ob)) return fail(MPYC_B200_EINVAL, "ff_all_any_axis: out overlaps the input");
+    return launch_status(launch_all_any_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, any != 0, (cudaStream_t)stream),
+                         "ff_all_any_axis launch");
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

@@ -18,6 +18,7 @@
 //   K8   k_copy_gather, k_copy_permute, k_binop_view (layout.cuh)   strided views, joins, broadcast arithmetic
 //   K11  k_inv_batch<NUM> (ff_div), k_select (select.cuh)   division and np.where       finfields.py:1199-1225
 //   K12  k_powexp_fixed, k_powexp_elem (powexp.cuh)   per-element exponents   finfields.py:1409-1414, gmpy.py:288-290
+//   K13  k_prod_*, k_cumprod_*, k_allany_* (prod.cuh)   np.prod / np.cumprod / np.all / np.any along any axis
 #pragma once
 #include "ff_arith.cuh"
 

@@ -112,6 +112,17 @@ cudaError_t launch_select(const FieldParams& fp, const unsigned char* mask, bool
 cudaError_t launch_powexp(const FieldParams& fp, const u64* a, const u64* tab, u32 tab_bytes, int w, int nwin, const u64* e,
                           int el, int ebits, const unsigned char* sgn, u64* out, size_t n, cudaStream_t st);
 
+// K13 (inst_prod.cu), on a C-ordered (O, R, I) array as K7: out (O, I) = init * prod_r in (O, R, I) (init: L canonical host
+// limbs, or null for 1); out (O, R + inc, I) = running products along R after a row of ones when inc; out (O, I) = 0 / 1
+// for all (any == false) or any element along R being nonzero.  in and out must not overlap.  Prime fields; sizes
+// validated by the caller.
+cudaError_t launch_prod_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, const u64* init,
+                             cudaStream_t st);
+cudaError_t launch_cumprod_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool inc,
+                                cudaStream_t st);
+cudaError_t launch_all_any_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool any,
+                                cudaStream_t st);
+
 extern template struct Launch<1>;
 extern template struct Launch<2>;
 extern template struct Launch<3>;

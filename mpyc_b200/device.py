@@ -472,6 +472,50 @@ def cumsum_axis(a: DeviceArray, shape, axis=None, include_initial=False):
     return out, out_shape
 
 
+def prod_axis(a: DeviceArray, shape, axis=None, keepdims=False, initial=1):
+    """np.prod(a.reshape(shape), axis=axis, keepdims=keepdims, initial=initial) mod p on the K13 kernels
+    (FiniteFieldArray.prod, mpyc/finfields.py:1339-1349).  axis: None, an int or a tuple, negative axes allowed; a tuple of
+    axes that are not adjacent is reduced one run of adjacent axes at a time, as sum_axis does.  Returns (DeviceArray of
+    the result's elements, result shape); a 0-d result is one element."""
+    from mpyc_b200 import axes
+    _check_elements(a, shape, 'prod_axis')
+    passes, out_shape = axes.sum_plan(shape, axis, keepdims)
+    init = a.ctx.scalar_limbs(int(initial) % a.ctx.order)
+    cur = a
+    for j, (O, R, I) in enumerate(passes):
+        out = DeviceArray.empty(a.ctx, O * I, a.t.device)
+        last = j == len(passes) - 1
+        check(lib.mpyc_b200_ff_prod_axis(a.ctx.handle, cur.ptr, O, R, I, init if last else None, out.ptr, _stream_ptr()))
+        cur = out
+    return cur, out_shape
+
+
+def cumprod_axis(a: DeviceArray, shape, axis=None, include_initial=False):
+    """np.cumprod(a.reshape(shape), axis) (axis=None: flattened) and, with include_initial, np.cumulative_prod(...,
+    include_initial=True) mod p on the K13 kernels.  Returns (DeviceArray, result shape)."""
+    from mpyc_b200 import axes
+    _check_elements(a, shape, 'cumprod_axis')
+    (O, R, I), out_shape = axes.scan_plan(shape, axis, include_initial)
+    out = DeviceArray.empty(a.ctx, O * (R + (1 if include_initial else 0)) * I, a.t.device)
+    check(lib.mpyc_b200_ff_cumprod_axis(a.ctx.handle, a.ptr, O, R, I, 1 if include_initial else 0, out.ptr, _stream_ptr()))
+    return out, out_shape
+
+
+def all_any_axis(a: DeviceArray, shape, axis=None, keepdims=False, any=False):
+    """np.all (any=False) / np.any (any=True) of a.reshape(shape) along axis, as field elements 0 / 1 (the reference's
+    `cls(bool_array)`, mpyc/finfields.py:766-819) on the K13 kernels.  Returns (DeviceArray, result shape).  A reduction to
+    one bool needs no kernel of its own: nonzero's count answers it."""
+    from mpyc_b200 import axes
+    _check_elements(a, shape, 'all_any_axis')
+    passes, out_shape = axes.sum_plan(shape, axis, keepdims)
+    cur = a
+    for O, R, I in passes:
+        out = DeviceArray.empty(a.ctx, O * I, a.t.device)
+        check(lib.mpyc_b200_ff_all_any_axis(a.ctx.handle, cur.ptr, O, R, I, 1 if any else 0, out.ptr, _stream_ptr()))
+        cur = out
+    return cur, out_shape
+
+
 def _view(v, index_keep):
     """mpyc_b200.layout.View -> the C struct (its index table stays alive in index_keep)."""
     c = _cabi.View()

@@ -140,7 +140,8 @@ def _install_gmpy(thresha_module):
 def _install_operators(finfields_module, min_size):
     """FiniteFieldArray.__init__ and + - * neg @ (mpyc/finfields.py:717-725,1056-1146): limb-backed operands, and plain
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
-    np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7) and np.outer (K1c) of such arrays.  Views, writes,
+    np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7), np.outer (K1c) and np.prod / FiniteFieldArray.prod,
+    np.cumprod, np.cumulative_prod, np.all, np.any (K13) of such arrays.  Views, writes,
     axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
     np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10.  / (reflected and in place),
     reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b, and ** and **=
@@ -152,7 +153,7 @@ def _install_operators(finfields_module, min_size):
     names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
              '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
              'sum', '__setitem__', 'transpose', 'swapaxes', '__truediv__', '__rtruediv__', '__itruediv__', 'reciprocal',
-             '__pow__', '__ipow__', 'sqrt', 'is_sqr')
+             '__pow__', '__ipow__', 'sqrt', 'is_sqr', 'prod')
     orig = {name: cls.__dict__[name] for name in names}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
@@ -160,8 +161,10 @@ def _install_operators(finfields_module, min_size):
     value_property = resident.make_value_property(finfields_module)
     slot_set = resident._slot.__set__
     import numpy as np
-    # np.sum / cumsum / cumulative_sum (K7) and np.outer (K1c), mpyc_b200.resident.array_function
-    reductions = tuple(f for f in (np.sum, np.cumsum, getattr(np, 'cumulative_sum', None), np.outer) if f is not None)
+    # np.sum / cumsum / cumulative_sum (K7), np.outer (K1c) and np.prod / cumprod / cumulative_prod / all / any (K13),
+    # mpyc_b200.resident.array_function
+    reductions = tuple(f for f in (np.sum, np.cumsum, getattr(np, 'cumulative_sum', None), np.outer, np.prod, np.cumprod,
+                                   getattr(np, 'cumulative_prod', None), np.all, np.any) if f is not None)
 
     def __init__(self, value, check=True, copy=False):
         lv = resident.as_limb_value(value)
@@ -261,6 +264,11 @@ def _install_operators(finfields_module, min_size):
         r = resident.array_function(self, np.sum, (self,) + args, kwargs) if len(args) <= 5 else MISS
         return orig['sum'](self, *args, **kwargs) if r is MISS else r
 
+    def prod(self, *args, **kwargs):
+        # ndarray.prod(axis=None, dtype=None, out=None, keepdims=False, initial=1, where=True)
+        r = resident.prod_method(self, args, kwargs)
+        return orig['prod'](self, *args, **kwargs) if r is MISS else r
+
     def __eq__(self, other):
         r = resident.equals(self, other, False)
         return orig['__eq__'](self, other) if r is MISS else r
@@ -322,6 +330,7 @@ def _install_operators(finfields_module, min_size):
     cls.swapaxes = swapaxes
     cls.__array_function__ = __array_function__
     cls.sum = sum
+    cls.prod = prod
     cls.__lshift__ = make_shift('__lshift__', False, False)
     cls.__rshift__ = make_shift('__rshift__', True, False)
     cls.__ilshift__ = make_shift('__ilshift__', False, True)

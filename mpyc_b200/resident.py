@@ -46,7 +46,7 @@ import sys
 
 resident = False      # np_recombine / PRSS results stay limb-backed (set by install(resident=True))
 min_size = 1024       # plain object-array operands of fewer elements are left to the reference's operators
-calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0}    # counters (tests, profiling)
+calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0, 'prod': 0}    # counters (tests, profiling)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -237,6 +237,21 @@ class CudaBackend:
         if not isinstance(base, int):
             base = self.to_store(ctx, base)
         return dev.pow_exp(ctx, base, exps, signs, bits, device=where)
+
+    # ---- K13, used by the np.prod / np.cumprod / np.all / np.any hooks ----
+    def prod_axis(self, ctx, a, shape, axis, keepdims, initial):
+        """store of the elements of np.prod(a.reshape(shape), axis, keepdims=keepdims, initial=initial) mod p"""
+        dev, _ = self._dev()
+        return dev.prod_axis(self.to_store(ctx, a), shape, axis, keepdims, initial)[0]
+
+    def cumprod_axis(self, ctx, a, shape, axis, include_initial):
+        dev, _ = self._dev()
+        return dev.cumprod_axis(self.to_store(ctx, a), shape, axis, include_initial)[0]
+
+    def all_any_axis(self, ctx, a, shape, axis, keepdims, any):
+        """store of np.all / np.any (any) of a.reshape(shape) along axis as elements 0 / 1"""
+        dev, _ = self._dev()
+        return dev.all_any_axis(self.to_store(ctx, a), shape, axis, keepdims, any)[0]
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -1562,13 +1577,16 @@ def matmul(self, other, reflected=False):
     return _wrap(cls, ctx, out, shape)
 
 
-def _reduction_operand(a):
+def _reduction_operand(a, ready=None):
     """(cls, ctx, store, shape) of a prime-field array that is limb-backed or an object array of at least min_size
-    elements (the rule of binop); None otherwise.  CudaBackend always has K7; a substituted backend without the sum_axis
-    / cumsum_axis pair (a test stand-in) leaves sums to the reference's code, as before K7 existed."""
+    elements (the rule of binop); None otherwise, and when the backend lacks the kernels (ready; default: K7's sum_axis /
+    cumsum_axis pair).  CudaBackend always has K7 and K13; a substituted backend without them (a test stand-in) leaves the
+    call to the reference's code, as before the kernels existed."""
+    if ready is None:
+        ready = hasattr(backend, 'cumsum_axis') and hasattr(backend, 'sum_axis')
     cls = type(a)
     ctx = _ctx_of(cls)
-    if ctx is None or ctx.binary or not hasattr(backend, 'cumsum_axis') or not hasattr(backend, 'sum_axis'):
+    if ctx is None or ctx.binary or not ready:
         return None
     mine = raw_value(a)
     if as_limb_value(mine) is None and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
@@ -1617,6 +1635,95 @@ def cumsum(a, axis=None, include_initial=False):
     return _wrap(cls, ctx, backend.cumsum_axis(ctx, store, shape, axis, bool(include_initial)), out_shape)
 
 
+_PROD_METHODS = ('prod_axis', 'cumprod_axis', 'all_any_axis')
+
+
+def _prod_backend():
+    """K13's hooks run only when the backend has prod_axis, cumprod_axis and all_any_axis.  CudaBackend always does; a
+    substituted backend without them (a test stand-in) leaves np.prod / np.cumprod / np.all / np.any to the reference's
+    code, as before K13 existed."""
+    return all(hasattr(backend, m) for m in _PROD_METHODS)
+
+
+def prod_(a, axis=None, keepdims=False, initial=1):
+    """np.prod(a, axis, keepdims=keepdims, initial=initial) / a.prod(...) (finfields.py:766-819,1339-1349) on the K13
+    kernels: a field element for a 0-d result, else a limb-backed array.  initial: a Python int (the caller turns a field
+    element into its value).  _MISS for bad axes (NumPy raises its own error), binary fields and arrays that are neither
+    limb-backed nor large."""
+    if type(initial) is not int or not isinstance(keepdims, (bool, np.bool_)):
+        return _MISS
+    try:
+        _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
+    except (TypeError, ValueError):
+        return _MISS
+    op = _reduction_operand(a, _prod_backend())
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    calls['prod'] += 1
+    out = backend.prod_axis(ctx, store, shape, axis, bool(keepdims), initial % ctx.modulus)
+    if out_shape == ():
+        calls['limb_ops'] += 1
+        return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
+    return _wrap(cls, ctx, out, out_shape)
+
+
+def cumprod(a, axis=None, include_initial=False):
+    """np.cumprod(a, axis) (axis=None: flattened) and np.cumulative_prod(a, axis=axis, include_initial=...) on the K13
+    running product; a limb-backed array, or _MISS as for prod_."""
+    try:
+        _, out_shape = axes.scan_plan(np.shape(raw_value(a)), axis, include_initial)
+    except (TypeError, ValueError):
+        return _MISS
+    op = _reduction_operand(a, _prod_backend())
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    calls['prod'] += 1
+    return _wrap(cls, ctx, backend.cumprod_axis(ctx, store, shape, axis, bool(include_initial)), out_shape)
+
+
+def all_any(a, axis=None, keepdims=False, any=False):
+    """np.all(a, axis, keepdims=keepdims) / np.any(...) (any) as the reference answers them (finfields.py:766-819): np.True_
+    or np.False_ for a 0-d result -- from the device's count of nonzero elements, nothing else crosses to the host -- else
+    a limb-backed array of 0 / 1 (the reference's `cls(bool_array)`) from the K13 kernels.  _MISS as for prod_."""
+    if not isinstance(keepdims, (bool, np.bool_)):
+        return _MISS
+    try:
+        _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
+    except (TypeError, ValueError):
+        return _MISS
+    op = _reduction_operand(a, _prod_backend())
+    if op is None:
+        return _MISS
+    cls, ctx, store, shape = op
+    calls['prod'] += 1
+    if out_shape == ():
+        _, count = backend.nonzero(ctx, store, want_mask=False)
+        n = layout._prod(shape)
+        return np.True_ if (count > 0 if any else count == n) else np.False_
+    return _wrap(cls, ctx, backend.all_any_axis(ctx, store, shape, axis, bool(keepdims), bool(any)), out_shape)
+
+
+def prod_method(self, args, kwargs):
+    """FiniteFieldArray.prod(*args, **kwargs) (finfields.py:1339-1349), which turns initial into a field element first:
+    an int or an element of the array's field is taken here, anything else (and initial or where given by position) stays
+    with the reference."""
+    names = ('axis', 'dtype', 'out', 'keepdims')
+    if (len(args) > len(names) or not set(kwargs) <= {'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'}
+            or set(kwargs) & set(names[:len(args)])):
+        return _MISS
+    bound = dict(zip(names, args), **kwargs)
+    if any(bound.get(k, None) is not None for k in ('dtype', 'out')) or 'where' in bound:
+        return _MISS
+    initial = bound.get('initial', 1)
+    if isinstance(initial, type(self).field):
+        initial = int(initial.value)
+    elif type(initial) is not int:
+        return _MISS
+    return prod_(self, bound.get('axis', None), bound.get('keepdims', False), initial)
+
+
 def outer(a, b):
     """np.outer(a, b) of two arrays of one prime field (Runtime.np_outer, runtime.py:2544-2578): c[i, j] = a_i b_j on the
     flattened operands, through K1c with k = 1.  _MISS for anything else -- a public integer operand in particular, whose
@@ -1644,17 +1751,20 @@ def outer(a, b):
 
 def array_function(self, func, args, kwargs):
     """The NumPy functions routed to K7 / K1c by FiniteFieldArray.__array_function__ (install._install_operators):
-    np.sum, np.cumsum, np.cumulative_sum, np.outer.  Arguments are bound as NumPy's signatures do; dtype / out / where
-    and unknown arguments leave the call to the reference (_MISS)."""
+    np.sum, np.cumsum, np.cumulative_sum, np.outer, and to K13: np.prod, np.cumprod, np.cumulative_prod, np.all, np.any.
+    Arguments are bound as NumPy's signatures do; dtype / out / where and unknown arguments leave the call to the
+    reference (_MISS)."""
     name = func.__name__
-    if name == 'cumulative_sum':
+    if name in ('cumulative_sum', 'cumulative_prod'):
         if len(args) != 1 or not set(kwargs) <= {'axis', 'include_initial', 'dtype', 'out'}:
             return _MISS
         bound = dict(kwargs, x=args[0])
         names = ('x',)
     else:
         names = {'sum': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'), 'cumsum': ('a', 'axis', 'dtype', 'out'),
-                 'outer': ('a', 'b', 'out')}.get(name)
+                 'outer': ('a', 'b', 'out'), 'prod': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'),
+                 'cumprod': ('a', 'axis', 'dtype', 'out'), 'all': ('a', 'axis', 'out', 'keepdims', 'where'),
+                 'any': ('a', 'axis', 'out', 'keepdims', 'where')}.get(name)
         if names is None or len(args) > len(names) or not set(kwargs) <= set(names[len(args):]):
             return _MISS
         bound = dict(zip(names, args), **kwargs)
@@ -1670,10 +1780,17 @@ def array_function(self, func, args, kwargs):
         return cumsum(first, opt('axis', None))
     if name == 'outer':
         return outer(first, bound.get('b'))
+    if name == 'prod':
+        return prod_(first, opt('axis', None), opt('keepdims', False), opt('initial', 1))
+    if name == 'cumprod':
+        return cumprod(first, opt('axis', None))
+    if name in ('all', 'any'):
+        return all_any(first, opt('axis', None), opt('keepdims', False), name == 'any')
     axis = opt('axis', None)
     if axis is None and np.ndim(raw_value(first)) > 1:
         return _MISS                      # NumPy requires the axis of a multi-dimensional array
-    return cumsum(first, axis, bool(opt('include_initial', False)))
+    scan = cumsum if name == 'cumulative_sum' else cumprod
+    return scan(first, axis, bool(opt('include_initial', False)))
 
 
 # the parameter names of the reference's implementations, so that keywords it rejects stay with it
