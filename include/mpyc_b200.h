@@ -270,6 +270,17 @@ int mpyc_b200_ff_cumprod_axis(const mpyc_b200_field* f, const void* d_in, size_t
 int mpyc_b200_ff_all_any_axis(const mpyc_b200_field* f, const void* d_in, size_t outer, size_t len, size_t inner, int any,
                               void* d_out, void* stream);
 
+/* ---- field matrix times public integer matrix (K14; prime fields) --------------------------------
+ * FiniteFieldArray @ an integer ndarray and back (mpyc/finfields.py:1126-1146; Runtime.np_argmax / np_argmin's
+ * `u @ np.arange(n)`, runtime.py:3750-3757, 3878-3885; np_matmul with a public operand, runtime.py:2482-2541).
+ * w_left == 0: C[r x c] = X[r x k] @ W[k x c] mod p; otherwise C[r x c] = W[r x k] @ X[k x c] mod p.  X: canonical residues
+ * (L limbs each); W: int64 entries, or uint64 when w_unsigned != 0, taken exactly (no reduction needed first).  All
+ * row-major and contiguous, 8-byte aligned (a matrix may start at any element of a larger buffer).  k == 0 writes zeros.
+ * MPYC_B200_EINVAL before any CUDA call for null buffers when the output is non-empty, byte counts that overflow,
+ * misaligned buffers and an output that overlaps an input; MPYC_B200_EUNSUPPORTED for binary fields. */
+int mpyc_b200_ff_matmul_int(const mpyc_b200_field* f, const void* d_x, const void* d_w, int w_unsigned, int w_left, void* d_c,
+                            size_t r, size_t k, size_t c, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -89,6 +89,8 @@ _SIGNATURES = {
     'mpyc_b200_ff_prod_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, POINTER(c_uint64), c_void_p, c_void_p]),
     'mpyc_b200_ff_cumprod_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p]),
     'mpyc_b200_ff_all_any_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p]),
+    'mpyc_b200_ff_matmul_int': (c_int, [_field_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_size_t, c_size_t,
+                                        c_void_p]),
     'mpyc_b200_ff_binop_rows': (c_int, [_field_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p]),
     'mpyc_b200_ff_conv2d': (c_int, [_field_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),

@@ -94,6 +94,38 @@ int mpyc_sm_count() {
     return sms > 0 ? sms : 132;
 }
 
+// Scratch for split partials (K13, K14), from a pool of the library's own that keeps its memory between calls: the device's
+// default pool returns freed memory at every synchronisation, and a fresh allocation cost a split call about 0.2 ms.
+// The partials take at most a few MB (about two waves of threads' worth of elements).
+cudaError_t mpyc_scratch_alloc(u64** p, size_t bytes, cudaStream_t st) {
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if (!pools[dev]) {
+            cudaMemPoolProps props = {};
+            props.allocType = cudaMemAllocationTypePinned;
+            props.location.type = cudaMemLocationTypeDevice;
+            props.location.id = dev;
+            cudaMemPool_t pool = nullptr;
+            e = cudaMemPoolCreate(&pool, &props);
+            if (e != cudaSuccess) return e;
+            uint64_t keep = UINT64_MAX;
+            e = cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+            if (e != cudaSuccess) {
+                cudaMemPoolDestroy(pool);
+                return e;
+            }
+            pools[dev] = pool;
+        }
+    }
+    return cudaMallocFromPoolAsync(reinterpret_cast<void**>(p), bytes, pools[dev], st);
+}
+
 // ---------------------------------------------------------------------------------------
 // field handle
 // ---------------------------------------------------------------------------------------
@@ -1130,6 +1162,34 @@ MPYC_API int mpyc_b200_ff_all_any_axis(const mpyc_b200_field* f, const void* d_i
     if (bytes_overlap(d_in, ib, d_out, ob)) return fail(MPYC_B200_EINVAL, "ff_all_any_axis: out overlaps the input");
     return launch_status(launch_all_any_axis(f->fp, (const u64*)d_in, (u64*)d_out, outer, len, inner, any != 0, (cudaStream_t)stream),
                          "ff_all_any_axis launch");
+}
+
+// ---------------------------------------------------------------------------------------
+// K14: field matrix times public 64-bit integer matrix (matmul_int.cuh; prime fields)
+// ---------------------------------------------------------------------------------------
+
+MPYC_API int mpyc_b200_ff_matmul_int(const mpyc_b200_field* f, const void* d_x, const void* d_w, int w_unsigned, int w_left,
+                                     void* d_c, size_t r, size_t k, size_t c, void* stream) {
+    if (int rc = prime_only(f, "ff_matmul_int: field is null")) return rc;
+    const size_t E = (size_t)f->fp.L * sizeof(u64);
+    size_t xe = 0, we = 0, xb = 0, wb = 0, cb = 0;
+    size_t rk = 0, kc = 0;
+    if (__builtin_mul_overflow(r, k, &rk) || __builtin_mul_overflow(k, c, &kc) || __builtin_mul_overflow(r, c, &cb))
+        return fail(MPYC_B200_EINVAL, "ff_matmul_int: size overflow");
+    xe = w_left ? kc : rk;
+    we = w_left ? rk : kc;
+    if (__builtin_mul_overflow(xe, E, &xb) || __builtin_mul_overflow(we, sizeof(u64), &wb) || __builtin_mul_overflow(cb, E, &cb) ||
+        xb > (size_t)INT64_MAX || wb > (size_t)INT64_MAX || cb > (size_t)INT64_MAX)
+        return fail(MPYC_B200_EINVAL, "ff_matmul_int: size overflow");
+    if (r == 0 || c == 0) return MPYC_B200_OK;
+    if (!d_c || (k && (!d_x || !d_w))) return fail(MPYC_B200_EINVAL, "ff_matmul_int: null buffer");
+    const uintptr_t any = reinterpret_cast<uintptr_t>(d_c) | (k ? reinterpret_cast<uintptr_t>(d_x) | reinterpret_cast<uintptr_t>(d_w) : 0);
+    if (any & 7u) return fail(MPYC_B200_EINVAL, "ff_matmul_int: buffers must be 8-byte aligned");
+    if (bytes_overlap(d_c, cb, d_x, xb) || bytes_overlap(d_c, cb, d_w, wb))
+        return fail(MPYC_B200_EINVAL, "ff_matmul_int: c overlaps an operand");
+    return launch_status(launch_matmul_int(f->fp, (const u64*)d_x, (const u64*)d_w, w_unsigned != 0, w_left != 0, (u64*)d_c, r, k, c,
+                                           (cudaStream_t)stream),
+                         "ff_matmul_int launch");
 }
 
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,

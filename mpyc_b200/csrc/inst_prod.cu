@@ -2,45 +2,12 @@
 // where the rows form would leave most lanes idle), the rows form otherwise; K7's 16-byte path for even L on 16-byte
 // aligned arrays.  R is split into slices when the shape's work items cannot fill two CTAs per SM (prod_plan); the slice
 // partials (S, O, I) live in stream-ordered scratch and are combined by a second pass of the same kernels on (1, S, O*I).
-#include <mutex>
 #include "launch_impl.cuh"
 #include "prod.cuh"
 
 namespace {
 
 bool cols_form(size_t R, size_t I) { return I >= 32 || R * I < 32; }
-
-// Scratch for the slice partials, from a pool of the library's own that keeps its memory between calls: the device's
-// default pool returns freed memory at every synchronisation, and a fresh allocation cost a split call about 0.2 ms.
-// The partials take at most a few MB (about two waves of threads' worth of elements).
-cudaError_t scratch_alloc(u64** p, size_t bytes, cudaStream_t st) {
-    static std::mutex mu;
-    static cudaMemPool_t pools[64] = {};
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        if (!pools[dev]) {
-            cudaMemPoolProps props = {};
-            props.allocType = cudaMemAllocationTypePinned;
-            props.location.type = cudaMemLocationTypeDevice;
-            props.location.id = dev;
-            cudaMemPool_t pool = nullptr;
-            e = cudaMemPoolCreate(&pool, &props);
-            if (e != cudaSuccess) return e;
-            uint64_t keep = UINT64_MAX;
-            e = cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-            if (e != cudaSuccess) {
-                cudaMemPoolDestroy(pool);
-                return e;
-            }
-            pools[dev] = pool;
-        }
-    }
-    return cudaMallocFromPoolAsync(reinterpret_cast<void**>(p), bytes, pools[dev], st);
-}
 
 // As K7's axis_plan, but for two CTAs per SM in both forms: a product thread holds more registers than a sum thread.
 // Slices keep >= 64 rows (columns) / >= 1024 elements (rows form).
@@ -125,7 +92,7 @@ cudaError_t prod_l(const FieldParams& fp, const u64* in, u64* out, size_t O, siz
     const AxisPlan pl = prod_plan(O, R, I);
     if (pl.S == 1) return prod_pass<L>(fp, in, out, O, R, I, 1, R, init, mul_init, st);
     u64* part = nullptr;                                 // (S, O, I) slice products, stream-ordered scratch
-    cudaError_t e = scratch_alloc(&part, pl.S * O * I * L * sizeof(u64), st);
+    cudaError_t e = mpyc_scratch_alloc(&part, pl.S * O * I * L * sizeof(u64), st);
     if (e != cudaSuccess) return e;
     e = prod_pass<L>(fp, in, part, O, R, I, pl.S, pl.rs, init, 0, st);
     if (e == cudaSuccess) e = prod_l<L>(fp, part, out, 1, pl.S, O * I, init, mul_init, st);
@@ -142,7 +109,7 @@ cudaError_t cumprod_l(const FieldParams& fp, const u64* in, u64* out, size_t O, 
     if (pl.S == 1) return cumprod_pass<L>(fp, in, out, O, R, I, 1, R, nullptr, inc, st);
     const size_t count = pl.S * O * I;
     u64* part = nullptr;                                 // slice products, then their running products
-    cudaError_t e = scratch_alloc(&part, 2 * count * L * sizeof(u64), st);
+    cudaError_t e = mpyc_scratch_alloc(&part, 2 * count * L * sizeof(u64), st);
     if (e != cudaSuccess) return e;
     const ScalarParam none = {};
     e = prod_pass<L>(fp, in, part, O, R, I, pl.S, pl.rs, none, 0, st);
@@ -159,7 +126,7 @@ cudaError_t allany_l(bool any, const u64* in, u64* out, size_t O, size_t R, size
     const AxisPlan pl = prod_plan(O, R, I);
     if (pl.S == 1) return allany_pass<L>(any, in, out, O, R, I, 1, R, st);
     u64* part = nullptr;
-    cudaError_t e = scratch_alloc(&part, pl.S * O * I * L * sizeof(u64), st);
+    cudaError_t e = mpyc_scratch_alloc(&part, pl.S * O * I * L * sizeof(u64), st);
     if (e != cudaSuccess) return e;
     e = allany_pass<L>(any, in, part, O, R, I, pl.S, pl.rs, st);
     if (e == cudaSuccess) e = allany_l<L>(any, part, out, 1, pl.S, O * I, st);

@@ -18,6 +18,10 @@ struct ShareDst {
 // persistent-grid sizing: enough CTAs to cover the items, capped at one full wave
 int mpyc_grid_size(const void* kernel, size_t items, size_t dyn_smem);
 
+// stream-ordered scratch for split partials from the library's per-device pool, which keeps its memory between calls
+// (api.cu); release with cudaFreeAsync on the same stream
+cudaError_t mpyc_scratch_alloc(u64** p, size_t bytes, cudaStream_t st);
+
 template <int L>
 struct Launch {
     // op in {OP_ADD, OP_SUB, OP_MUL, OP_NEG}; scal != nullptr -> broadcast second operand (host limbs)
@@ -122,6 +126,11 @@ cudaError_t launch_cumprod_axis(const FieldParams& fp, const u64* in, u64* out, 
                                 cudaStream_t st);
 cudaError_t launch_all_any_axis(const FieldParams& fp, const u64* in, u64* out, size_t O, size_t R, size_t I, bool any,
                                 cudaStream_t st);
+
+// K14 (inst_matmul_int.cu): C (r x c) = X (r x k) @ W (k x c), or with w_left W (r x k) @ X (k x c), mod p; X canonical
+// field elements, W 64-bit integers (int64, or uint64 when w_unsigned).  Prime fields; sizes validated by the caller.
+cudaError_t launch_matmul_int(const FieldParams& fp, const u64* X, const u64* W, bool w_unsigned, bool w_left, u64* C, size_t r,
+                              size_t k, size_t c, cudaStream_t st);
 
 extern template struct Launch<1>;
 extern template struct Launch<2>;

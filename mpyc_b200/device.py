@@ -325,6 +325,28 @@ def matmul(ctx, A, B, r, k, c):
     return out
 
 
+def matmul_int(ctx, X, w, r, k, c, w_left=False):
+    """C = X @ W mod p, or W @ X with w_left, on the K14 kernels: X a row-major DeviceArray of r*k (w_left: k*c) field
+    elements, w a NumPy integer array of k*c (w_left: r*k) entries (FiniteFieldArray @ an integer ndarray,
+    mpyc/finfields.py:1126-1146).  The entries go to the device as 64-bit integers, never as Python ints: int8 ... int64 and
+    uint8 ... uint32 as int64, uint64 as itself with the kernel's unsigned flag.  Returns a DeviceArray of r*c elements."""
+    w = np.asarray(w)
+    if w.dtype.kind not in 'iu':
+        raise TypeError(f'matmul_int: integer entries expected, not {w.dtype}')
+    unsigned = w.dtype == np.uint64
+    buf = np.ascontiguousarray(w).view(np.int64) if unsigned else np.ascontiguousarray(w, dtype=np.int64)
+    if X.n != (k * c if w_left else r * k) or buf.size != (r * k if w_left else k * c):
+        raise ValueError('matmul_int: shapes do not match the buffers')
+    X._check_contiguous()
+    if not buf.flags.writeable:           # torch.from_numpy warns about read-only arrays
+        buf = buf.copy()
+    W = torch.from_numpy(buf.reshape(-1)).to(X.t.device)
+    out = DeviceArray.empty(ctx, r * c, X.t.device)
+    check(lib.mpyc_b200_ff_matmul_int(ctx.handle, X.ptr, ctypes.c_void_p(W.data_ptr()), 1 if unsigned else 0,
+                                      1 if w_left else 0, out.ptr, r, k, c, _stream_ptr()))
+    return out
+
+
 # ---- protocol-local algebra on raw share values (SURVEY 8f N3 / N4; csrc/local.cuh) -----------------------------
 
 def fma(a: DeviceArray, b, c: DeviceArray):

@@ -141,8 +141,9 @@ def _install_operators(finfields_module, min_size):
     """FiniteFieldArray.__init__ and + - * neg @ (mpyc/finfields.py:717-725,1056-1146): limb-backed operands, and plain
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
     np.sum / FiniteFieldArray.sum, np.cumsum, np.cumulative_sum (K7), np.outer (K1c) and np.prod / FiniteFieldArray.prod,
-    np.cumprod, np.cumulative_prod, np.all, np.any (K13) of such arrays.  Views, writes,
-    axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
+    np.cumprod, np.cumulative_prod, np.all, np.any (K13) of such arrays; np.matmul of field arrays runs on K1c as @ does, and
+    with install(public_matmul=True) @ and np.matmul with an ndarray of a NumPy integer dtype on either side run on K14.
+    Views, writes, axis permutations, joins, flips, rolls and broadcast + - * of limb-backed arrays run on K8 (mpyc_b200.layout), and
     np.linalg.det / solve / inv / matrix_power on K9 and K1c, and np.convolve on K10.  / (reflected and in place),
     reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b, and ** and **=
     by an integer array of the same shape on K12; everything
@@ -153,7 +154,7 @@ def _install_operators(finfields_module, min_size):
     names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
              '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
              'sum', '__setitem__', 'transpose', 'swapaxes', '__truediv__', '__rtruediv__', '__itruediv__', 'reciprocal',
-             '__pow__', '__ipow__', 'sqrt', 'is_sqr', 'prod')
+             '__pow__', '__ipow__', 'sqrt', 'is_sqr', 'prod', '__array_ufunc__')
     orig = {name: cls.__dict__[name] for name in names}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
@@ -194,6 +195,20 @@ def _install_operators(finfields_module, min_size):
     def __rmatmul__(self, other):
         r = resident.matmul(self, other, reflected=True)
         return orig['__rmatmul__'](self, other) if r is MISS else r
+
+    def __array_ufunc__(self, ufunc, method, *inputs, **kwargs):
+        # np.matmul(x, y) with two positional operands -- `int_ndarray @ field_array`, `object_ndarray @ field_array` and
+        # np.matmul of field arrays, which NumPy hands to __array_ufunc__ (finfields.py:728-764) -- goes where @ goes:
+        # K14 for a NumPy integer operand, K1c otherwise.  Other ufuncs, methods and keywords, and ndarray subclasses, run
+        # the reference's method.
+        if ufunc is np.matmul and method == '__call__' and not kwargs and len(inputs) == 2 and \
+                all(isinstance(x, cls) or type(x) is np.ndarray for x in inputs):
+            left = isinstance(inputs[0], cls)
+            mine, other = (inputs[0], inputs[1]) if left else (inputs[1], inputs[0])
+            r = resident.matmul(mine, other, reflected=not left, ufunc=True)
+            if r is not MISS:
+                return r
+        return orig['__array_ufunc__'](self, ufunc, method, *inputs, **kwargs)
 
     def make_shift(name, right, inplace):
         # `a << n` = a * 2^n, `a >> n` = a * (2^n)^-1 for an integer n (finfields.py:1227-1271); limb-backed arrays only
@@ -346,10 +361,12 @@ def _install_operators(finfields_module, min_size):
     cls.__neg__ = __neg__
     cls.__matmul__ = __matmul__
     cls.__rmatmul__ = __rmatmul__
+    cls.__array_ufunc__ = __array_ufunc__
 
 
 def install(thresha_module=None, strict=False, device=0, finfields_module=None, finfields_min_size=256,
-            limb_wire=False, min_size=0, operators=False, operators_min_size=1024, resident=False, local_algebra=True):
+            limb_wire=False, min_size=0, operators=False, operators_min_size=1024, resident=False, local_algebra=True,
+            public_matmul=False):
     """Patch `mpyc.thresha` (or the module passed in); with finfields_module also the batched
     inverse/pow/sqrt/is_sqr of PrimeFieldArray.  limb_wire=True: shares travel between parties as limb
     buffers (mpyc_b200.wire; every party must run mpyc_b200).  min_size > 0: calls on fewer elements are left to
@@ -361,6 +378,10 @@ def install(thresha_module=None, strict=False, device=0, finfields_module=None, 
     where a value is actually looked at (input, output, raw-value arithmetic).  local_algebra (with resident): the raw-value
     arithmetic of Runtime.np_random_bits / np_trunc / np_sgn runs mod p on the device as well (resident.ModValue, K6 kernels).
     resident=True also routes mpyc.gmpy.powmod_exp_list (2 ** x, np_pow, np_exp2, np_exp of secure arrays) to K12.
+    public_matmul (with operators or resident): @ and np.matmul of a field array with an ndarray of a NumPy integer dtype
+    run on K14 (np_matmul with public weights, the `u @ np.arange(n)` of np_argmax / np_argmin / np_unit_vector), so the
+    field operand stays limb-backed; without it those products settle the field operand and run the reference's code, as
+    before K14, and the conversion counts of existing programs stay what they were.
     Returns the list of patched names."""
     if thresha_module is None:
         import mpyc.thresha as thresha_module
@@ -375,6 +396,7 @@ def install(thresha_module=None, strict=False, device=0, finfields_module=None, 
     from mpyc_b200 import resident as res
     res.resident = bool(resident)
     res.local_algebra = bool(local_algebra and resident)
+    res.public_matmul = bool(public_matmul)
     res.backend.device = device
     engine.device = device
     engine.limb_wire = bool(limb_wire or resident)
@@ -400,6 +422,7 @@ def uninstall():
     engine.limb_wire = False
     from mpyc_b200 import resident as res
     res.resident = False
+    res.public_matmul = False
     if _saved_ops:
         cls = _saved_ops.pop('cls')
         res.restore_value_slot(_saved_ops.pop('module'))

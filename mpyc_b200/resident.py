@@ -46,7 +46,9 @@ import sys
 
 resident = False      # np_recombine / PRSS results stay limb-backed (set by install(resident=True))
 min_size = 1024       # plain object-array operands of fewer elements are left to the reference's operators
-calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0, 'prod': 0}    # counters (tests, profiling)
+public_matmul = False  # @ / np.matmul with a NumPy integer ndarray run on K14 (set by install(public_matmul=True))
+calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0, 'prod': 0,
+         'matmul_int': 0}    # counters (tests, profiling)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -252,6 +254,12 @@ class CudaBackend:
         """store of np.all / np.any (any) of a.reshape(shape) along axis as elements 0 / 1"""
         dev, _ = self._dev()
         return dev.all_any_axis(self.to_store(ctx, a), shape, axis, keepdims, any)[0]
+
+    # ---- K14, used by matmul with an integer ndarray operand ----
+    def matmul_int(self, ctx, x, w, r, k, c, w_left):
+        """store of x @ w (w_left: w @ x) mod p, x a store of r*k (w_left: k*c) elements, w a NumPy integer array"""
+        dev, _ = self._dev()
+        return dev.matmul_int(ctx, self.to_store(ctx, x), w, r, k, c, w_left)
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -1538,8 +1546,16 @@ def negate(self):
     return _wrap(cls, ctx, backend.neg(ctx, a[0]), a[1])
 
 
-def matmul(self, other, reflected=False):
-    """self @ other (reflected: other @ self) for 1-D / 2-D operands through K1c."""
+def _int_matrix(x):
+    """A plain ndarray of a NumPy integer dtype: K14's public operand."""
+    return type(x) is np.ndarray and x.dtype.kind in 'iu'
+
+
+def matmul(self, other, reflected=False, ufunc=False):
+    """self @ other (reflected: other @ self) for 1-D / 2-D operands: through K14 when the other operand is an ndarray of a
+    NumPy integer dtype, public_matmul is set and the backend has matmul_int, through K1c otherwise.  ufunc: the call is
+    np.matmul through __array_ufunc__, whose 1-D @ 1-D result is a 0-d array (the reference's `cls(a)`,
+    finfields.py:760-764) rather than a field element."""
     cls = type(self)
     ctx = _ctx_of(cls)
     if ctx is None:
@@ -1559,20 +1575,33 @@ def matmul(self, other, reflected=False):
     limbish = any(isinstance(x, cls) and as_limb_value(raw_value(x)) is not None for x in (A, B))
     if not limbish and r * k * c < min_size * 8:
         return _MISS
+    public = _int_matrix(other)
+    if public and (not public_matmul or ctx.binary or not hasattr(backend, 'matmul_int')):
+        return _MISS
     saved = min_size
     try:
         globals()['min_size'] = 0         # both operands are packed whatever their size
-        a = _operand(ctx, cls, A)
-        b = _operand(ctx, cls, B)
+        if public:
+            x = _operand(ctx, cls, self)
+        else:
+            a = _operand(ctx, cls, A)
+            b = _operand(ctx, cls, B)
     finally:
         globals()['min_size'] = saved
-    if a is None or b is None:
-        return _MISS
-    out = backend.matmul(ctx, a[0], b[0], r, k, c)
+    if public:
+        if x is None:
+            return _MISS
+        calls['matmul_int'] += 1
+        out = backend.matmul_int(ctx, x[0], other, r, k, c, reflected)
+    else:
+        if a is None or b is None:
+            return _MISS
+        out = backend.matmul(ctx, a[0], b[0], r, k, c)
     if len(sa) == 1 and len(sb) == 1:     # inner product: a field element (finfields.py:1134)
         calls['limb_ops'] += 1
         poly = type(cls.field.modulus) if ctx.binary else None
-        return cls.field(LimbValue(ctx, out, (1,), poly)._materialise()[0])
+        v = LimbValue(ctx, out, (1,), poly)._materialise()[0]
+        return cls(np.array(v, dtype=object), check=False) if ufunc else cls.field(v)
     shape = (c,) if len(sa) == 1 else ((r,) if len(sb) == 1 else (r, c))
     return _wrap(cls, ctx, out, shape)
 
