@@ -14,7 +14,7 @@ restatement of the kernels, and without a CUDA device it raises.
 """
 import functools
 
-from mpyc_b200 import thresha as engine
+from mpyc_b200 import _cabi, thresha as engine
 from mpyc_b200._cabi import UnsupportedFieldError
 from mpyc_b200.field import context_of_field
 
@@ -137,6 +137,41 @@ def _install_gmpy(thresha_module):
     gmpy.powmod_exp_list = powmod_exp_list
 
 
+# FiniteFieldArray method -> (hook in mpyc_b200.resident, fixed keyword arguments of the hook)
+_HOOKS = {
+    '__add__': ('binop', {'op': _cabi.OP_ADD}),
+    '__radd__': ('binop', {'op': _cabi.OP_ADD}),
+    '__sub__': ('binop', {'op': _cabi.OP_SUB}),
+    '__rsub__': ('binop', {'op': _cabi.OP_SUB, 'reflected': True}),
+    '__mul__': ('binop', {'op': _cabi.OP_MUL}),
+    '__rmul__': ('binop', {'op': _cabi.OP_MUL}),
+    '__neg__': ('negate', {}),
+    '__matmul__': ('matmul', {}),
+    '__rmatmul__': ('matmul', {'reflected': True}),
+    '__lshift__': ('shift', {'right': False}),
+    '__rshift__': ('shift', {'right': True}),
+    '__ilshift__': ('shift', {'right': False}),
+    '__irshift__': ('shift', {'right': True}),
+    '__getitem__': ('getitem', {}),
+    '__setitem__': ('setitem', {}),
+    'transpose': ('transpose', {}),
+    'swapaxes': ('swapaxes', {}),
+    '__eq__': ('equals', {'negate': False}),
+    '__ne__': ('equals', {'negate': True}),
+    '__truediv__': ('divide', {}),
+    '__rtruediv__': ('divide', {'reflected': True}),
+    '__itruediv__': ('divide', {}),
+    'reciprocal': ('reciprocal', {}),
+    '__pow__': ('power', {}),
+    '__ipow__': ('power', {}),
+    'sqrt': ('sqrt', {}),
+    'is_sqr': ('is_sqr', {}),
+    'prod': ('prod_method', {}),
+}
+# in-place operators give self a new store: arrays sharing the old one keep their values
+_INPLACE = ('__ilshift__', '__irshift__', '__itruediv__', '__ipow__')
+
+
 def _install_operators(finfields_module, min_size):
     """FiniteFieldArray.__init__ and + - * neg @ (mpyc/finfields.py:717-725,1056-1146): limb-backed operands, and plain
     object arrays of at least `min_size` elements, are combined by the K1 / K1c kernels (mpyc_b200.resident), and so are
@@ -148,24 +183,32 @@ def _install_operators(finfields_module, min_size):
     reciprocal, ** and **= by an int, sqrt (Blum primes), is_sqr and np.where(cond, x, y) run on K11 and K1b, and ** and **=
     by an integer array of the same shape on K12; everything
     else -- scalars with small arrays, uncovered fields and keys -- runs the reference's own method unchanged."""
-    from mpyc_b200 import _cabi, resident
+    from mpyc_b200 import resident
+    import numpy as np
     resident.min_size = int(min_size)
     cls = finfields_module.FiniteFieldArray
-    names = ('__init__', '__add__', '__radd__', '__sub__', '__rsub__', '__mul__', '__rmul__', '__neg__', '__matmul__',
-             '__rmatmul__', '__lshift__', '__rshift__', '__ilshift__', '__irshift__', '__getitem__', '__array_function__', '__eq__', '__ne__',
-             'sum', '__setitem__', 'transpose', 'swapaxes', '__truediv__', '__rtruediv__', '__itruediv__', 'reciprocal',
-             '__pow__', '__ipow__', 'sqrt', 'is_sqr', 'prod', '__array_ufunc__')
-    orig = {name: cls.__dict__[name] for name in names}
+    orig = {name: cls.__dict__[name] for name in ('__init__', *_HOOKS, '__array_function__', 'sum', '__array_ufunc__')}
     _saved_ops.update({'cls': cls, 'module': finfields_module, **orig})
     MISS = resident._MISS
     orig_hash = cls.__hash__          # assigning __eq__ on a class does not touch __hash__, kept explicit for clarity
     value_property = resident.make_value_property(finfields_module)
     slot_set = resident._slot.__set__
-    import numpy as np
-    # np.sum / cumsum / cumulative_sum (K7), np.outer (K1c) and np.prod / cumprod / cumulative_prod / all / any (K13),
-    # mpyc_b200.resident.array_function
-    reductions = tuple(f for f in (np.sum, np.cumsum, getattr(np, 'cumulative_sum', None), np.outer, np.prod, np.cumprod,
-                                   getattr(np, 'cumulative_prod', None), np.all, np.any) if f is not None)
+
+    def hooked(name, hook, fixed):
+        # the hook is looked up in resident when called, so that rebinding it there takes effect
+        inplace = name in _INPLACE
+
+        def method(self, *args, **kwargs):
+            r = getattr(resident, hook)(self, *args, **kwargs, **fixed)
+            if r is MISS:
+                return orig[name](self, *args, **kwargs)
+            if inplace:
+                slot_set(self, resident.raw_value(r))
+                return self
+            return r
+        method.__name__ = name
+        method.__doc__ = orig[name].__doc__
+        return method
 
     def __init__(self, value, check=True, copy=False):
         lv = resident.as_limb_value(value)
@@ -175,26 +218,6 @@ def _install_operators(finfields_module, min_size):
         if type(value) is resident.LimbValue or type(value) is resident.ModValue:
             value = value._ints        # already an object array (canonical residues)
         orig['__init__'](self, value, check=check, copy=copy)
-
-    def make(op, name, reflected=False):
-        def method(self, other):
-            r = resident.binop(self, other, op, reflected)
-            return orig[name](self, other) if r is MISS else r
-        method.__name__ = name
-        method.__doc__ = orig[name].__doc__
-        return method
-
-    def __neg__(self):
-        r = resident.negate(self)
-        return orig['__neg__'](self) if r is MISS else r
-
-    def __matmul__(self, other):
-        r = resident.matmul(self, other)
-        return orig['__matmul__'](self, other) if r is MISS else r
-
-    def __rmatmul__(self, other):
-        r = resident.matmul(self, other, reflected=True)
-        return orig['__rmatmul__'](self, other) if r is MISS else r
 
     def __array_ufunc__(self, ufunc, method, *inputs, **kwargs):
         # np.matmul(x, y) with two positional operands -- `int_ndarray @ field_array`, `object_ndarray @ field_array` and
@@ -210,157 +233,22 @@ def _install_operators(finfields_module, min_size):
                 return r
         return orig['__array_ufunc__'](self, ufunc, method, *inputs, **kwargs)
 
-    def make_shift(name, right, inplace):
-        # `a << n` = a * 2^n, `a >> n` = a * (2^n)^-1 for an integer n (finfields.py:1227-1271); limb-backed arrays only
-        def method(self, other):
-            r = resident.shift(self, other, right)
-            if r is MISS:
-                return orig[name](self, other)
-            if inplace:
-                slot_set(self, resident.raw_value(r))
-                return self
-            return r
-        method.__name__ = name
-        method.__doc__ = orig[name].__doc__
-        return method
-
-    def __getitem__(self, key):
-        r = resident.getitem(self, key)
-        return orig['__getitem__'](self, key) if r is MISS else r
-
-    def __setitem__(self, key, value):
-        if resident.setitem(self, key, value) is MISS:
-            orig['__setitem__'](self, key, value)
-
-    def transpose(self, *axes):
-        # T is self.transpose() (finfields.py:1366-1368)
-        r = resident.permute(self, lambda nd: resident.layout.transpose_axes(nd, axes))
-        return orig['transpose'](self, *axes) if r is MISS else r
-
-    def swapaxes(self, axis1, axis2):
-        r = resident.permute(self, lambda nd: resident.layout.swapaxes_axes(nd, axis1, axis2))
-        return orig['swapaxes'](self, axis1, axis2) if r is MISS else r
-
     def __array_function__(self, func, types, args, kwargs):
-        import numpy as np
-        if func in resident.LAYOUT_FUNCTIONS and isinstance(self, cls):
-            r = resident.layout_function(type(self), func, args, kwargs)
-            if r is not MISS:
-                return r
-        if (func is np.concatenate and isinstance(self, cls) and len(args) == 1 and set(kwargs) <= {'axis'}
-                and not resident._layout_backend()):                   # without K8: axis-0 joins of limb-backed arrays
-            r = resident.concatenate(type(self), list(args[0]), kwargs.get('axis', 0))
-            if r is not MISS:
-                return r
-        if func in reductions and isinstance(self, cls):
-            r = resident.array_function(self, func, args, kwargs)
-            if r is not MISS:
-                return r
-        if func in resident.LINALG_FUNCTIONS and isinstance(self, cls):
-            r = resident.linalg_function(type(self), func, args, kwargs)
-            if r is not MISS:
-                return r
-        if func is np.convolve and isinstance(self, cls):
-            r = resident.convolve(type(self), args, kwargs)
-            if r is not MISS:
-                return r
-        if func is np.where:
-            # a field element that comes first in np.where's arguments hands the call over with self the element
-            # (FiniteFieldElement.__array_function__, finfields.py:83-85)
-            klass = type(self) if isinstance(self, cls) else getattr(type(self), 'array', None)
-            if isinstance(klass, type) and issubclass(klass, cls):
-                r = resident.where(klass, args, kwargs)
-                if r is not MISS:
-                    return r
-        return orig['__array_function__'](self, func, types, args, kwargs)
+        r = resident.array_function(self, func, args, kwargs)
+        return orig['__array_function__'](self, func, types, args, kwargs) if r is MISS else r
 
     def sum(self, *args, **kwargs):
         # ndarray.sum(axis=None, dtype=None, out=None, keepdims=False, initial=0, where=True)
-        r = resident.array_function(self, np.sum, (self,) + args, kwargs) if len(args) <= 5 else MISS
+        r = resident.reduction_function(self, np.sum, (self,) + args, kwargs) if len(args) <= 5 else MISS
         return orig['sum'](self, *args, **kwargs) if r is MISS else r
 
-    def prod(self, *args, **kwargs):
-        # ndarray.prod(axis=None, dtype=None, out=None, keepdims=False, initial=1, where=True)
-        r = resident.prod_method(self, args, kwargs)
-        return orig['prod'](self, *args, **kwargs) if r is MISS else r
-
-    def __eq__(self, other):
-        r = resident.equals(self, other, False)
-        return orig['__eq__'](self, other) if r is MISS else r
-
-    def __ne__(self, other):
-        r = resident.equals(self, other, True)
-        return orig['__ne__'](self, other) if r is MISS else r
-
-    def make_inplace(name, fn):
-        # `/=` and `**=` give self a new store, as `<<=` does: arrays sharing the old one keep their values
-        def method(self, other):
-            r = fn(self, other)
-            if r is MISS:
-                return orig[name](self, other)
-            slot_set(self, resident.raw_value(r))
-            return self
-        method.__name__ = name
-        method.__doc__ = orig[name].__doc__
-        return method
-
-    def __truediv__(self, other):
-        r = resident.divide(self, other)
-        return orig['__truediv__'](self, other) if r is MISS else r
-
-    def __rtruediv__(self, other):
-        r = resident.divide(self, other, reflected=True)
-        return orig['__rtruediv__'](self, other) if r is MISS else r
-
-    def reciprocal(self):
-        r = resident.reciprocal(self)
-        return orig['reciprocal'](self) if r is MISS else r
-
-    def __pow__(self, other):
-        r = resident.power(self, other)
-        return orig['__pow__'](self, other) if r is MISS else r
-
-    def sqrt(self, INV=False):
-        r = resident.sqrt(self, INV)
-        return orig['sqrt'](self, INV=INV) if r is MISS else r
-
-    def is_sqr(self):
-        r = resident.is_sqr(self)
-        return orig['is_sqr'](self) if r is MISS else r
-
-    cls.__truediv__ = __truediv__
-    cls.__rtruediv__ = __rtruediv__
-    cls.__itruediv__ = make_inplace('__itruediv__', resident.divide)
-    cls.reciprocal = reciprocal
-    cls.__pow__ = __pow__
-    cls.__ipow__ = make_inplace('__ipow__', resident.power)
-    cls.sqrt = sqrt
-    cls.is_sqr = is_sqr
-    cls.__eq__ = __eq__
-    cls.__ne__ = __ne__
+    for name, (hook, fixed) in _HOOKS.items():
+        setattr(cls, name, hooked(name, hook, fixed))
     cls.__hash__ = orig_hash
-    cls.__getitem__ = __getitem__
-    cls.__setitem__ = __setitem__
-    cls.transpose = transpose
-    cls.swapaxes = swapaxes
     cls.__array_function__ = __array_function__
     cls.sum = sum
-    cls.prod = prod
-    cls.__lshift__ = make_shift('__lshift__', False, False)
-    cls.__rshift__ = make_shift('__rshift__', True, False)
-    cls.__ilshift__ = make_shift('__ilshift__', False, True)
-    cls.__irshift__ = make_shift('__irshift__', True, True)
     cls.value = value_property
     cls.__init__ = __init__
-    cls.__add__ = make(_cabi.OP_ADD, '__add__')
-    cls.__radd__ = make(_cabi.OP_ADD, '__radd__')
-    cls.__sub__ = make(_cabi.OP_SUB, '__sub__')
-    cls.__rsub__ = make(_cabi.OP_SUB, '__rsub__', reflected=True)
-    cls.__mul__ = make(_cabi.OP_MUL, '__mul__')
-    cls.__rmul__ = make(_cabi.OP_MUL, '__rmul__')
-    cls.__neg__ = __neg__
-    cls.__matmul__ = __matmul__
-    cls.__rmatmul__ = __rmatmul__
     cls.__array_ufunc__ = __array_ufunc__
 
 

@@ -1161,8 +1161,9 @@ def _ctx_of(cls):
         return None
 
 
-def _operand(ctx, cls, x, want_shape=None):
-    """(store, shape) of an array operand as limbs, or None when it should stay with the reference's code."""
+def _operand(ctx, cls, x, any_size=False):
+    """(store, shape) of an array operand as limbs, or None when it should stay with the reference's code.  An object array
+    of Python ints is packed when it has at least min_size elements, or whatever its size with any_size."""
     if isinstance(x, cls):
         x = raw_value(x)
     lv = as_limb_value(x)
@@ -1170,10 +1171,15 @@ def _operand(ctx, cls, x, want_shape=None):
         return (lv.store, lv.shape) if lv.ctx is ctx else None
     if type(x) is LimbValue or type(x) is ModValue:
         x = x._ints
-    if isinstance(x, np.ndarray) and x.dtype == object and x.size >= min_size and not ctx.binary:
+    if isinstance(x, np.ndarray) and x.dtype == object and (any_size or x.size >= min_size) and not ctx.binary:
         calls['packed'] += 1
         return codec.ints_to_limbs(x.reshape(-1), ctx), x.shape
     return None
+
+
+def _qualifies(value):
+    """The operand rule of the hooks: a raw value that is limb-backed, or an ndarray of at least min_size elements."""
+    return as_limb_value(value) is not None or (isinstance(value, np.ndarray) and value.size >= min_size)
 
 
 def _gf2_mod(a, f):
@@ -1210,9 +1216,7 @@ def binop(self, other, op, reflected=False):
     ctx = _ctx_of(cls)
     if ctx is None:
         return _MISS
-    mine = raw_value(self)
-    big_or_limbs = as_limb_value(mine) is not None or (isinstance(mine, np.ndarray) and mine.size >= min_size)
-    if not big_or_limbs and not (isinstance(other, cls) and as_limb_value(raw_value(other)) is not None):
+    if not _qualifies(raw_value(self)) and not (isinstance(other, cls) and as_limb_value(raw_value(other)) is not None):
         return _MISS
     a = _operand(ctx, cls, self)
     if a is None:
@@ -1346,14 +1350,11 @@ def setitem(self, key, value):
         return _MISS
     if isinstance(value, cls):
         vv = raw_value(value)
-        vlv = as_limb_value(vv)
-        if vlv is not None and vlv.ctx is ctx:
-            vstore, vshape = vlv.store, vlv.shape
-        elif isinstance(vv, np.ndarray) and vv.dtype == object and not ctx.binary:
-            calls['packed'] += 1
-            vstore, vshape = codec.ints_to_limbs(vv.reshape(-1), ctx), vv.shape
-        else:
+        # a settled LimbValue in the slot is left to the reference, which settles the slot itself
+        op = None if type(vv) is LimbValue and vv.store is None else _operand(ctx, cls, vv, any_size=True)
+        if op is None:
             return _MISS
+        vstore, vshape = op
     else:
         k = _scalar(ctx, cls, value)
         if k is None:
@@ -1390,9 +1391,18 @@ def permute(self, order):
     return _view_result(cls, lv, view, view.shape)
 
 
+def transpose(self, *axes):
+    """self.transpose(*axes) (T is self.transpose(), finfields.py:1358-1368) on K8, as permute."""
+    return permute(self, lambda nd: layout.transpose_axes(nd, axes))
+
+
+def swapaxes(self, axis1, axis2):
+    return permute(self, lambda nd: layout.swapaxes_axes(nd, axis1, axis2))
+
+
 def _join_parts(cls, arrays):
-    """[(store, shape)] of a join's pieces -- arrays of class cls, limb-backed or (prime fields) of Python ints, which are
-    packed, at least one limb-backed -- or None."""
+    """[(shape, LimbValue or None)] of a join's pieces -- arrays of class cls, limb-backed or (prime fields) of Python ints
+    (None), at least one limb-backed -- or None."""
     if not isinstance(arrays, (list, tuple)) or not arrays or any(type(a) is not cls for a in arrays):
         return None
     ctx = _ctx_of(cls)
@@ -1403,20 +1413,20 @@ def _join_parts(cls, arrays):
     parts = []
     for v, x in zip(lvs, vals):
         if v is not None:
-            parts.append((v.store, v.shape, v._poly))
+            parts.append((v.shape, v))
         elif isinstance(x, np.ndarray) and x.dtype == object and not ctx.binary:
-            parts.append((None, x.shape, x))
+            parts.append((x.shape, None))
         else:
             return None
     return parts
 
 
-def _pack(ctx, part):
-    store, shape, x = part
-    if store is not None:
-        return store
-    calls['packed'] += 1
-    return codec.ints_to_limbs(x.reshape(-1), ctx)
+def _bind(names, args, kwargs):
+    """{parameter: argument} of args and kwargs bound to the parameter names `names` in order; None for more args than
+    names, and for a keyword that is unknown or repeats a positional argument."""
+    if len(args) > len(names) or not set(kwargs) <= set(names[len(args):]):
+        return None
+    return dict(zip(names, args), **kwargs)
 
 
 _LAYOUT_PARAMS = {'transpose': ('a', 'axes'), 'swapaxes': ('a', 'axis1', 'axis2'), 'moveaxis': ('a', 'source', 'destination'),
@@ -1434,10 +1444,8 @@ def layout_function(cls, func, args, kwargs):
     arguments, 0-d results and arguments NumPy rejects give _MISS."""
     name = func.__name__
     names = _LAYOUT_PARAMS.get(name)
-    if names is None or len(args) > len(names) or not set(kwargs) <= set(names[len(args):]) or not _layout_backend():
-        return _MISS
-    bound = dict(zip(names, args), **kwargs)
-    if len(bound) < _LAYOUT_REQUIRED.get(name, 1):
+    bound = None if names is None else _bind(names, args, kwargs)
+    if bound is None or not _layout_backend() or len(bound) < _LAYOUT_REQUIRED.get(name, 1):
         return _MISS
     first = bound[names[0]]
     try:
@@ -1445,7 +1453,7 @@ def layout_function(cls, func, args, kwargs):
             parts = _join_parts(cls, first)
             if parts is None:
                 return _MISS
-            shapes = [p[1] for p in parts]
+            shapes = [p[0] for p in parts]
             if name == 'concatenate':
                 out_shape, items = layout.concatenate_plan(shapes, bound.get('axis', 0))
             elif name == 'stack':
@@ -1457,8 +1465,8 @@ def layout_function(cls, func, args, kwargs):
             if not out_shape:
                 return _MISS
             ctx = _ctx_of(cls)
-            stores = [_pack(ctx, p) for p in parts]
-            poly = next(p[2] for p in parts if p[0] is not None)
+            stores = [_operand(ctx, cls, a, any_size=True)[0] for a in first]
+            poly = next(v._poly for _, v in parts if v is not None)
             lv = LimbValue(ctx, stores[0], shapes[0], poly)
             return _gather(cls, lv, [(stores[i], s, d) for i, s, d in items], out_shape)
         if type(first) is not cls:
@@ -1467,11 +1475,11 @@ def layout_function(cls, func, args, kwargs):
         if lv is None:
             return _MISS
         shape = lv.shape
-        if name in ('transpose', 'swapaxes', 'moveaxis'):
-            if name == 'transpose':
-                return permute(first, lambda nd: layout.transpose_axes(nd, (bound.get('axes'),)))
-            if name == 'swapaxes':
-                return permute(first, lambda nd: layout.swapaxes_axes(nd, bound['axis1'], bound['axis2']))
+        if name == 'transpose':
+            return transpose(first, bound.get('axes'))
+        if name == 'swapaxes':
+            return swapaxes(first, bound['axis1'], bound['axis2'])
+        if name == 'moveaxis':
             return permute(first, lambda nd: layout.moveaxis_axes(nd, bound['source'], bound['destination']))
         if name in ('expand_dims', 'squeeze'):
             out_shape = layout.reshaped(shape, func, bound.get('axis'))
@@ -1491,9 +1499,13 @@ def layout_function(cls, func, args, kwargs):
         return _MISS
 
 
-def concatenate(cls, arrays, axis):
-    """np.concatenate(arrays, axis=0) of limb-backed arrays of one field (np_prod's odd step, runtime.py:2202); _MISS otherwise."""
-    if axis != 0 or not arrays:
+def concatenate(cls, args, kwargs):
+    """np.concatenate(arrays, axis=0) of limb-backed arrays of one field (np_prod's odd step, runtime.py:2202) on a backend
+    without K8, which layout_function covers; _MISS otherwise."""
+    if len(args) != 1 or not set(kwargs) <= {'axis'} or _layout_backend():
+        return _MISS
+    arrays = list(args[0])
+    if kwargs.get('axis', 0) != 0 or not arrays:
         return _MISS
     lvs = [as_limb_value(raw_value(a)) if isinstance(a, cls) else None for a in arrays]
     if any(v is None or v.ctx is not lvs[0].ctx or v.shape[1:] != lvs[0].shape[1:] or not v.shape for v in lvs):
@@ -1578,22 +1590,14 @@ def matmul(self, other, reflected=False, ufunc=False):
     public = _int_matrix(other)
     if public and (not public_matmul or ctx.binary or not hasattr(backend, 'matmul_int')):
         return _MISS
-    saved = min_size
-    try:
-        globals()['min_size'] = 0         # both operands are packed whatever their size
-        if public:
-            x = _operand(ctx, cls, self)
-        else:
-            a = _operand(ctx, cls, A)
-            b = _operand(ctx, cls, B)
-    finally:
-        globals()['min_size'] = saved
     if public:
+        x = _operand(ctx, cls, self, any_size=True)
         if x is None:
             return _MISS
         calls['matmul_int'] += 1
         out = backend.matmul_int(ctx, x[0], other, r, k, c, reflected)
     else:
+        a, b = _operand(ctx, cls, A, any_size=True), _operand(ctx, cls, B, any_size=True)
         if a is None or b is None:
             return _MISS
         out = backend.matmul(ctx, a[0], b[0], r, k, c)
@@ -1606,22 +1610,23 @@ def matmul(self, other, reflected=False, ufunc=False):
     return _wrap(cls, ctx, out, shape)
 
 
-def _reduction_operand(a, ready=None):
-    """(cls, ctx, store, shape) of a prime-field array that is limb-backed or an object array of at least min_size
-    elements (the rule of binop); None otherwise, and when the backend lacks the kernels (ready; default: K7's sum_axis /
-    cumsum_axis pair).  CudaBackend always has K7 and K13; a substituted backend without them (a test stand-in) leaves the
-    call to the reference's code, as before the kernels existed."""
-    if ready is None:
-        ready = hasattr(backend, 'cumsum_axis') and hasattr(backend, 'sum_axis')
+def _array_operand(a, ready, nonempty=False):
+    """(cls, ctx, store, shape) of a prime-field array that meets the operand rule (_qualifies); None otherwise, when the
+    backend lacks the hook's kernels (ready: the hook's capability gate) and, with nonempty, for an empty array."""
     cls = type(a)
     ctx = _ctx_of(cls)
-    if ctx is None or ctx.binary or not ready:
-        return None
-    mine = raw_value(a)
-    if as_limb_value(mine) is None and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
+    if ctx is None or ctx.binary or not ready or not _qualifies(raw_value(a)):
         return None
     op = _operand(ctx, cls, a)
-    return None if op is None else (cls, ctx) + op
+    if op is None or (nonempty and not layout._prod(op[1])):
+        return None
+    return (cls, ctx) + op
+
+
+def _sum_backend():
+    """K7's hooks run only when the backend has sum_axis and cumsum_axis.  CudaBackend always does; a substituted backend
+    without them (a test stand-in) leaves the call to the reference's code, as before K7 existed."""
+    return hasattr(backend, 'cumsum_axis') and hasattr(backend, 'sum_axis')
 
 
 def _plain_int(x):
@@ -1639,15 +1644,12 @@ def sum_(a, axis=None, keepdims=False, initial=0):
         _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
     except (TypeError, ValueError):
         return _MISS
-    op = _reduction_operand(a)
+    op = _array_operand(a, _sum_backend())
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
     out = backend.sum_axis(ctx, store, shape, axis, bool(keepdims), int(initial) % ctx.modulus)
-    if out_shape == ():
-        calls['limb_ops'] += 1
-        return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
-    return _wrap(cls, ctx, out, out_shape)
+    return _element(cls, ctx, out) if out_shape == () else _wrap(cls, ctx, out, out_shape)
 
 
 def cumsum(a, axis=None, include_initial=False):
@@ -1657,7 +1659,7 @@ def cumsum(a, axis=None, include_initial=False):
         _, out_shape = axes.scan_plan(np.shape(raw_value(a)), axis, include_initial)
     except (TypeError, ValueError):
         return _MISS
-    op = _reduction_operand(a)
+    op = _array_operand(a, _sum_backend())
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
@@ -1685,16 +1687,13 @@ def prod_(a, axis=None, keepdims=False, initial=1):
         _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
     except (TypeError, ValueError):
         return _MISS
-    op = _reduction_operand(a, _prod_backend())
+    op = _array_operand(a, _prod_backend())
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
     calls['prod'] += 1
     out = backend.prod_axis(ctx, store, shape, axis, bool(keepdims), initial % ctx.modulus)
-    if out_shape == ():
-        calls['limb_ops'] += 1
-        return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
-    return _wrap(cls, ctx, out, out_shape)
+    return _element(cls, ctx, out) if out_shape == () else _wrap(cls, ctx, out, out_shape)
 
 
 def cumprod(a, axis=None, include_initial=False):
@@ -1704,7 +1703,7 @@ def cumprod(a, axis=None, include_initial=False):
         _, out_shape = axes.scan_plan(np.shape(raw_value(a)), axis, include_initial)
     except (TypeError, ValueError):
         return _MISS
-    op = _reduction_operand(a, _prod_backend())
+    op = _array_operand(a, _prod_backend())
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
@@ -1722,7 +1721,7 @@ def all_any(a, axis=None, keepdims=False, any=False):
         _, out_shape = axes.sum_plan(np.shape(raw_value(a)), axis, keepdims)
     except (TypeError, ValueError):
         return _MISS
-    op = _reduction_operand(a, _prod_backend())
+    op = _array_operand(a, _prod_backend())
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
@@ -1734,16 +1733,12 @@ def all_any(a, axis=None, keepdims=False, any=False):
     return _wrap(cls, ctx, backend.all_any_axis(ctx, store, shape, axis, bool(keepdims), bool(any)), out_shape)
 
 
-def prod_method(self, args, kwargs):
+def prod_method(self, *args, **kwargs):
     """FiniteFieldArray.prod(*args, **kwargs) (finfields.py:1339-1349), which turns initial into a field element first:
     an int or an element of the array's field is taken here, anything else (and initial or where given by position) stays
     with the reference."""
-    names = ('axis', 'dtype', 'out', 'keepdims')
-    if (len(args) > len(names) or not set(kwargs) <= {'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'}
-            or set(kwargs) & set(names[:len(args)])):
-        return _MISS
-    bound = dict(zip(names, args), **kwargs)
-    if any(bound.get(k, None) is not None for k in ('dtype', 'out')) or 'where' in bound:
+    bound = _bind(('axis', 'dtype', 'out', 'keepdims', 'initial', 'where'), args, kwargs) if len(args) <= 4 else None
+    if bound is None or any(bound.get(k, None) is not None for k in ('dtype', 'out')) or 'where' in bound:
         return _MISS
     initial = bound.get('initial', 1)
     if isinstance(initial, type(self).field):
@@ -1766,38 +1761,31 @@ def outer(a, b):
     na, nb = int(np.size(va)), int(np.size(vb))
     if not limbish and na * nb < min_size:
         return _MISS
-    saved = min_size
-    try:
-        globals()['min_size'] = 0         # both operands are packed whatever their size
-        x = _operand(ctx, cls, a)
-        y = _operand(ctx, cls, b)
-    finally:
-        globals()['min_size'] = saved
+    x, y = _operand(ctx, cls, a, any_size=True), _operand(ctx, cls, b, any_size=True)
     if x is None or y is None:
         return _MISS
     return _wrap(cls, ctx, backend.matmul(ctx, x[0], y[0], na, 1, nb), (na, nb))
 
 
-def array_function(self, func, args, kwargs):
-    """The NumPy functions routed to K7 / K1c by FiniteFieldArray.__array_function__ (install._install_operators):
-    np.sum, np.cumsum, np.cumulative_sum, np.outer, and to K13: np.prod, np.cumprod, np.cumulative_prod, np.all, np.any.
-    Arguments are bound as NumPy's signatures do; dtype / out / where and unknown arguments leave the call to the
-    reference (_MISS)."""
+_REDUCTION_PARAMS = {'sum': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'), 'cumsum': ('a', 'axis', 'dtype', 'out'),
+                     'outer': ('a', 'b', 'out'), 'prod': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'),
+                     'cumprod': ('a', 'axis', 'dtype', 'out'), 'all': ('a', 'axis', 'out', 'keepdims', 'where'),
+                     'any': ('a', 'axis', 'out', 'keepdims', 'where'),
+                     'cumulative_sum': ('x', 'axis', 'include_initial', 'dtype', 'out'),
+                     'cumulative_prod': ('x', 'axis', 'include_initial', 'dtype', 'out')}
+REDUCTION_FUNCTIONS = tuple(getattr(np, name) for name in _REDUCTION_PARAMS if hasattr(np, name))
+
+
+def reduction_function(self, func, args, kwargs):
+    """The NumPy functions routed to K7 / K1c by array_function and FiniteFieldArray.sum: np.sum, np.cumsum,
+    np.cumulative_sum, np.outer, and to K13: np.prod, np.cumprod, np.cumulative_prod, np.all, np.any.  Arguments are bound
+    as NumPy's signatures do (the cumulative ones take x by position only, the rest by keyword); dtype / out / where and
+    unknown arguments leave the call to the reference (_MISS)."""
     name = func.__name__
-    if name in ('cumulative_sum', 'cumulative_prod'):
-        if len(args) != 1 or not set(kwargs) <= {'axis', 'include_initial', 'dtype', 'out'}:
-            return _MISS
-        bound = dict(kwargs, x=args[0])
-        names = ('x',)
-    else:
-        names = {'sum': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'), 'cumsum': ('a', 'axis', 'dtype', 'out'),
-                 'outer': ('a', 'b', 'out'), 'prod': ('a', 'axis', 'dtype', 'out', 'keepdims', 'initial', 'where'),
-                 'cumprod': ('a', 'axis', 'dtype', 'out'), 'all': ('a', 'axis', 'out', 'keepdims', 'where'),
-                 'any': ('a', 'axis', 'out', 'keepdims', 'where')}.get(name)
-        if names is None or len(args) > len(names) or not set(kwargs) <= set(names[len(args):]):
-            return _MISS
-        bound = dict(zip(names, args), **kwargs)
-    if any(bound.get(k, None) is not None for k in ('dtype', 'out')) or bound.get('where', np._NoValue) is not np._NoValue:
+    names = _REDUCTION_PARAMS[name]
+    bound = None if name.startswith('cumulative_') and len(args) != 1 else _bind(names, args, kwargs)
+    if bound is None or any(bound.get(k, None) is not None for k in ('dtype', 'out')) or \
+            bound.get('where', np._NoValue) is not np._NoValue:
         return _MISS
     first = bound.get(names[0])
     if type(first) is not type(self):
@@ -1822,6 +1810,32 @@ def array_function(self, func, args, kwargs):
     return scan(first, axis, bool(opt('include_initial', False)))
 
 
+def array_function(self, func, args, kwargs):
+    """FiniteFieldArray.__array_function__ (finfields.py:766-819) on the kernels, or _MISS for the reference's method.  The
+    hooks are looked up when called and tried in this order: layout functions (K8), np.concatenate without K8, sums and
+    products (K7, K1c, K13), linear algebra (K9), np.convolve (K10) and np.where (K11).  self is an array of the patched
+    class or, for np.where only, a field element whose `array` is such a class: FiniteFieldElement.__array_function__
+    hands the call over with self the element (finfields.py:83-85)."""
+    cls = _array_class(self)
+    if cls is None:
+        klass = getattr(type(self), 'array', None)
+        if func is np.where and isinstance(klass, type) and issubclass(klass, _slot.__objclass__):
+            return where(klass, args, kwargs)
+        return _MISS
+    if func in LAYOUT_FUNCTIONS:
+        r = layout_function(cls, func, args, kwargs)
+        return concatenate(cls, args, kwargs) if r is _MISS and func is np.concatenate else r
+    if func in REDUCTION_FUNCTIONS:
+        return reduction_function(self, func, args, kwargs)
+    if func in LINALG_FUNCTIONS:
+        return linalg_function(cls, func, args, kwargs)
+    if func is np.convolve:
+        return convolve(cls, args, kwargs)
+    if func is np.where:
+        return where(cls, args, kwargs)
+    return _MISS
+
+
 # the parameter names of the reference's implementations, so that keywords it rejects stay with it
 _LINALG_PARAMS = {'det': ('a',), 'solve': ('A', 'B'), 'inv': ('A',), 'matrix_power': ('A', 'n')}
 LINALG_FUNCTIONS = tuple(getattr(np.linalg, name) for name in _LINALG_PARAMS)
@@ -1843,10 +1857,8 @@ def linalg_function(cls, func, args, kwargs):
     unknown arguments."""
     name = func.__name__
     names = _LINALG_PARAMS[name]
-    if len(args) > len(names) or not set(kwargs) <= set(names[len(args):]) or not _linalg_backend():
-        return _MISS
-    bound = dict(zip(names, args), **kwargs)
-    if len(bound) != len(names):
+    bound = _bind(names, args, kwargs)
+    if bound is None or not _linalg_backend() or len(bound) != len(names):
         return _MISS
     ctx = _ctx_of(cls)
     A, B = bound[names[0]], bound.get('B')
@@ -1870,21 +1882,13 @@ def linalg_function(cls, func, args, kwargs):
     limbish = any(as_limb_value(raw_value(x)) is not None for x in operands)
     if not limbish and np.size(raw_value(A)) < min_size:
         return _MISS
-    saved = min_size
-    try:
-        globals()['min_size'] = 0         # both operands are packed whatever their size
-        ops = [_operand(ctx, cls, x) for x in operands]
-    finally:
-        globals()['min_size'] = saved
+    ops = [_operand(ctx, cls, x, any_size=True) for x in operands]
     if any(o is None for o in ops):
         return _MISS
     a = ops[0][0]
     if name == 'det':
         out = backend.det(ctx, a, batch, n)
-        if len(shape) == 2:
-            calls['limb_ops'] += 1
-            return cls.field(int(codec.limbs_to_ints(backend.to_host(ctx, out), ctx)[0]))
-        return _wrap(cls, ctx, out, shape[:-2])
+        return _element(cls, ctx, out) if len(shape) == 2 else _wrap(cls, ctx, out, shape[:-2])
     if name == 'solve':
         nrhs = ops[1][1][1]
         return _wrap(cls, ctx, backend.solve(ctx, a, n, ops[1][0], nrhs), (n, nrhs))
@@ -1947,17 +1951,12 @@ def convolve(cls, args, kwargs):
     if not limbish and m * n < min_size:
         return _MISS
     stores = [None, None]
-    saved = min_size
-    try:
-        globals()['min_size'] = 0         # both operands are packed whatever their size
-        for k, x in enumerate(operands):
-            if public[k] is None:
-                op = _operand(ctx, cls, x)
-                if op is None:
-                    return _MISS
-                stores[k] = op[0]
-    finally:
-        globals()['min_size'] = saved
+    for k, x in enumerate(operands):
+        if public[k] is None:
+            op = _operand(ctx, cls, x, any_size=True)
+            if op is None:
+                return _MISS
+            stores[k] = op[0]
     for k, ints in enumerate(public):
         if ints is not None:
             calls['packed'] += 1
@@ -1973,22 +1972,6 @@ def _divsel_backend():
     """K11's hooks run only when the backend has divide and select.  CudaBackend always does; a substituted backend without
     them (a test stand-in) leaves division and selection to the reference's code, as before K11 existed."""
     return hasattr(backend, 'divide') and hasattr(backend, 'select')
-
-
-def _unary_operand(a):
-    """(cls, ctx, store, shape) of a prime-field array that is limb-backed or an object array of at least min_size elements
-    (the rule of binop), not empty; None otherwise, and always without K11."""
-    cls = type(a)
-    ctx = _ctx_of(cls)
-    if ctx is None or ctx.binary or not _divsel_backend():
-        return None
-    mine = raw_value(a)
-    if as_limb_value(mine) is None and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
-        return None
-    op = _operand(ctx, cls, a)
-    if op is None or not layout._prod(op[1]):
-        return None
-    return (cls, ctx) + op
 
 
 def _public_scalar(cls, x):
@@ -2025,8 +2008,7 @@ def divide(self, other, reflected=False):
     k = _public_scalar(cls, other)
     if k is None and not reflected and type(other) is cls:
         mine, theirs = raw_value(self), raw_value(other)
-        limbish = as_limb_value(mine) is not None or as_limb_value(theirs) is not None
-        if not limbish and not (isinstance(mine, np.ndarray) and mine.size >= min_size):
+        if not _qualifies(mine) and as_limb_value(theirs) is None:
             return _MISS
         if np.shape(mine) != np.shape(theirs) or not layout._prod(np.shape(mine)):
             return _MISS
@@ -2040,7 +2022,7 @@ def divide(self, other, reflected=False):
         return _wrap(cls, ctx, out, a[1])
     if k is None:
         return _MISS
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None:
         return _MISS
     _, _, store, shape = op
@@ -2059,7 +2041,7 @@ def divide(self, other, reflected=False):
 
 def reciprocal(self):
     """self.reciprocal() (finfields.py:1278-1281) on ff_inv: a limb-backed array, or _MISS as for divide."""
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
@@ -2078,7 +2060,7 @@ def power(self, e):
         return power_exp(self, e)
     if type(e) is not int:
         return _MISS
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None:
         return _MISS
     cls, ctx, store, shape = op
@@ -2111,7 +2093,7 @@ def power_exp(self, e):
     other dtypes, exponents wider than 256 bits, negative exponents, binary fields and backends without K12."""
     if not _powexp_backend():
         return _MISS
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None or e.shape != op[3]:
         return _MISS
     cls, ctx, store, shape = op
@@ -2151,7 +2133,7 @@ def powmod_exp_list(base, exp_lst, mod):
 def sqrt(self, INV=False):
     """self.sqrt(INV) for Blum primes (PrimeFieldArray._sqrt, finfields.py:1424-1438) on K1b; INV with a zero raises the
     reference's ZeroDivisionError('no inverse sqrt of 0').  _MISS for other primes and as for divide."""
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None or not isinstance(INV, bool):
         return _MISS
     cls, ctx, store, shape = op
@@ -2167,7 +2149,7 @@ def sqrt(self, INV=False):
 def is_sqr(self):
     """self.is_sqr() (finfields.py:1298-1300, 1463-1470) on K1b: a host bool ndarray of the array's shape (0 counts as a
     square).  _MISS for 0-d arrays and as for divide."""
-    op = _unary_operand(self)
+    op = _array_operand(self, _divsel_backend(), nonempty=True)
     if op is None or not op[3]:
         return _MISS
     cls, ctx, store, shape = op
@@ -2186,11 +2168,7 @@ def where(cls, args, kwargs):
     cond, x, y = args
     if type(cond) is not np.ndarray:
         return _MISS
-    arrays = [v for v in (x, y) if type(v) is cls]
-    if not arrays:
-        return _MISS
-    vals = [raw_value(v) for v in arrays]
-    if all(as_limb_value(v) is None for v in vals) and not any(isinstance(v, np.ndarray) and v.size >= min_size for v in vals):
+    if not any(type(v) is cls and _qualifies(raw_value(v)) for v in (x, y)):
         return _MISS
     r = _where(ctx, cls, cond, x, y)
     return _MISS if r is None else r
@@ -2208,12 +2186,7 @@ def conv2d(x, W, b):
     sx, sw, sb = (getattr(raw_value(a), 'shape', None) for a in (x, W, b))
     if len(sx) != 4 or len(sw) != 4 or len(sb) != 1 or sx[1] != sw[1] or sw[2] != sw[3] or sb[0] != sw[0]:
         raise ValueError(f'conv2d: shapes {sx}, {sw}, {sb} do not fit (k,r,m,n), (v,r,s,s), (v,)')
-    saved = min_size
-    try:
-        globals()['min_size'] = 0
-        ops = [_operand(ctx, cls, a) for a in (x, W, b)]
-    finally:
-        globals()['min_size'] = saved
+    ops = [_operand(ctx, cls, a, any_size=True) for a in (x, W, b)]
     if any(o is None for o in ops):
         raise _cabi.UnsupportedFieldError('conv2d: operands must be limb-backed or object arrays of the field')
     k, r, m, n = sx
