@@ -281,6 +281,26 @@ int mpyc_b200_ff_all_any_axis(const mpyc_b200_field* f, const void* d_in, size_t
 int mpyc_b200_ff_matmul_int(const mpyc_b200_field* f, const void* d_x, const void* d_w, int w_unsigned, int w_left, void* d_c,
                             size_t r, size_t k, size_t c, void* stream);
 
+/* ---- GF(2^8) bit composition, broadcast arithmetic and stacked products (K15) --------------------
+ * Elements are single bytes (canonical: the field polynomial has degree 8).  Any byte alignment works.  Each entry point
+ * returns MPYC_B200_EUNSUPPORTED for prime fields, and MPYC_B200_EINVAL before any CUDA call for null buffers, bad shapes,
+ * byte counts that overflow and an output that overlaps an input.
+ *
+ * d_out[i] = sum_j d_bits[i l + j] X^j mod poly for i < n, j < l (l >= 1): np.sum(v << np.arange(l), axis=-1) of
+ * BinaryPolynomial values followed by field.array(...) (Runtime.np_to_bits' r_modl and np_from_bits, mpyc/runtime.py:4415,
+ * 4483). */
+int mpyc_b200_gf_bits_compose(const mpyc_b200_field* f, const void* d_bits, size_t n, size_t l, void* d_out, void* stream);
+/* out = a (op) b under NumPy broadcasting, op ADD or SUB (both XOR) or MUL: the views and out as for
+ * mpyc_b200_ff_binop_view (FiniteFieldArray + - * of GF(2^8) arrays of two shapes, mpyc/finfields.py:1056-1124). */
+int mpyc_b200_gf_binop_view(const mpyc_b200_field* f, int op, const void* d_a, size_t a_len, const mpyc_b200_view* a,
+                            const void* d_b, size_t b_len, const mpyc_b200_view* b, void* d_out, void* stream);
+/* C[b] (r x c) = A[b] (r x k) @ B[b] (k x c) for b < batch, all row-major; A[b] = d_a + b * a_batch_stride, likewise B,
+ * and C[b] = d_c + b r c.  A batch stride is 0 (one matrix for every b: NumPy's matmul broadcast) or the matrix size (r k
+ * for A, k c for B).  A broadcast A of at most 4096 entries is held in shared memory: the AES S-box's A @ x[..., None]
+ * (demos/np_aes.py) is one launch.  k == 0 writes zeros. */
+int mpyc_b200_gf_matmul_batched(const mpyc_b200_field* f, const void* d_a, size_t a_batch_stride, const void* d_b,
+                                size_t b_batch_stride, void* d_c, size_t batch, size_t r, size_t k, size_t c, void* stream);
+
 /* Y[k][v][m][n] = B[v] + 'same' 2-D correlation of X[k][r][m][n] with W[v][r][s][s] summed over the r input channels,
  * mod p, s odd -- demos/np_cnnmnist.py:69-81 (convolvetensor's np.correlate loops followed by field.array(Y)).
  * All arrays contiguous, row-major. */

@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, '_obj')
 LIB = os.path.join(HERE, 'libmpyc_b200.so')
 SOURCES = ['api.cu', 'inst_L1.cu', 'inst_L2.cu', 'inst_L3.cu', 'inst_L4.cu', 'inst_layout.cu', 'inst_linalg.cu', 'inst_conv.cu',
-           'inst_select.cu', 'inst_powexp.cu', 'inst_prod.cu', 'inst_matmul_int.cu']
+           'inst_select.cu', 'inst_powexp.cu', 'inst_prod.cu', 'inst_matmul_int.cu', 'inst_gf.cu']
 HOST_SOURCES = ['shake128_x8.cpp']   # host compiler only (AVX-512 through per-function target attributes)
 PUBLIC_HEADER = os.path.join('..', '..', 'include', 'mpyc_b200.h')
 

@@ -91,6 +91,11 @@ _SIGNATURES = {
     'mpyc_b200_ff_all_any_axis': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p]),
     'mpyc_b200_ff_matmul_int': (c_int, [_field_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_size_t, c_size_t,
                                         c_void_p]),
+    'mpyc_b200_gf_bits_compose': (c_int, [_field_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    'mpyc_b200_gf_binop_view': (c_int, [_field_p, c_int, c_void_p, c_size_t, _view_p, c_void_p, c_size_t, _view_p, c_void_p,
+                                        c_void_p]),
+    'mpyc_b200_gf_matmul_batched': (c_int, [_field_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t,
+                                            c_size_t, c_size_t, c_void_p]),
     'mpyc_b200_ff_binop_rows': (c_int, [_field_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p]),
     'mpyc_b200_ff_conv2d': (c_int, [_field_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),

@@ -1192,6 +1192,71 @@ MPYC_API int mpyc_b200_ff_matmul_int(const mpyc_b200_field* f, const void* d_x, 
                          "ff_matmul_int launch");
 }
 
+// ---------------------------------------------------------------------------------------
+// K15: GF(2^8) bit composition, broadcast arithmetic and stacked products (gf_local.cuh)
+// ---------------------------------------------------------------------------------------
+
+static int gf_only(const mpyc_b200_field* f, const char* what) {
+    if (!f) return fail(MPYC_B200_EINVAL, what);
+    if (f->kind != MPYC_B200_KIND_GF256) return fail(MPYC_B200_EUNSUPPORTED, "K15 kernels cover GF(2^8) only");
+    return MPYC_B200_OK;
+}
+
+MPYC_API int mpyc_b200_gf_bits_compose(const mpyc_b200_field* f, const void* d_bits, size_t n, size_t l, void* d_out, void* stream) {
+    if (int rc = gf_only(f, "gf_bits_compose: field is null")) return rc;
+    if (l == 0) return fail(MPYC_B200_EINVAL, "gf_bits_compose: l must be at least 1");
+    size_t ib = 0;
+    if (__builtin_mul_overflow(n, l, &ib) || ib > (size_t)INT64_MAX) return fail(MPYC_B200_EINVAL, "gf_bits_compose: size overflow");
+    if (n == 0) return MPYC_B200_OK;
+    if (!d_bits || !d_out) return fail(MPYC_B200_EINVAL, "gf_bits_compose: null buffer");
+    if (bytes_overlap(d_bits, ib, d_out, n)) return fail(MPYC_B200_EINVAL, "gf_bits_compose: out overlaps the input");
+    return launch_status(launch_gf_bits_compose(f->gf_poly, (const unsigned char*)d_bits, n, l, (unsigned char*)d_out,
+                                                (cudaStream_t)stream),
+                         "gf_bits_compose launch");
+}
+
+MPYC_API int mpyc_b200_gf_binop_view(const mpyc_b200_field* f, int op, const void* d_a, size_t a_len, const mpyc_b200_view* a,
+                                     const void* d_b, size_t b_len, const mpyc_b200_view* b, void* d_out, void* stream) {
+    if (int rc = gf_only(f, "gf_binop_view: field is null")) return rc;
+    if (op < 0 || op > 2) return fail(MPYC_B200_EINVAL, "gf_binop_view: op must be ADD, SUB or MUL");
+    const long long na = view_check(a, a_len, false), nb = view_check(b, b_len, false);
+    if (na < 0 || nb < 0) return fail(MPYC_B200_EINVAL, "gf_binop_view: bad view (rank > 6, negative extent, index table or outside its buffer)");
+    if (!same_extents(a, b)) return fail(MPYC_B200_EINVAL, "gf_binop_view: views of different extents");
+    if (na == 0) return MPYC_B200_OK;
+    if (!d_a || !d_b || !d_out) return fail(MPYC_B200_EINVAL, "gf_binop_view: null buffer");
+    if (bytes_overlap(d_out, (size_t)na, d_a, a_len) || bytes_overlap(d_out, (size_t)na, d_b, b_len))
+        return fail(MPYC_B200_EINVAL, "gf_binop_view: out overlaps an operand");
+    BinopPlan p = {};
+    p.rank = a->rank;
+    p.aoff = a->offset, p.boff = b->offset;
+    for (int k = 0; k < p.rank; k++) p.ext[k] = a->extent[k], p.astr[k] = a->stride[k], p.bstr[k] = b->stride[k];
+    if (p.rank == 0) p.rank = 1, p.ext[0] = 1;
+    return launch_status(launch_gf_binop_view(f->gf_poly, op, p, (const unsigned char*)d_a, (const unsigned char*)d_b,
+                                              (unsigned char*)d_out, (cudaStream_t)stream),
+                         "gf_binop_view launch");
+}
+
+MPYC_API int mpyc_b200_gf_matmul_batched(const mpyc_b200_field* f, const void* d_a, size_t a_batch_stride, const void* d_b,
+                                         size_t b_batch_stride, void* d_c, size_t batch, size_t r, size_t k, size_t c, void* stream) {
+    if (int rc = gf_only(f, "gf_matmul_batched: field is null")) return rc;
+    size_t rk = 0, kc = 0, rc_ = 0, ab = 0, bb = 0, cb = 0;
+    if (__builtin_mul_overflow(r, k, &rk) || __builtin_mul_overflow(k, c, &kc) || __builtin_mul_overflow(r, c, &rc_) ||
+        __builtin_mul_overflow(rc_, batch, &cb) || cb > (size_t)INT64_MAX)
+        return fail(MPYC_B200_EINVAL, "gf_matmul_batched: size overflow");
+    if ((a_batch_stride != 0 && a_batch_stride != rk) || (b_batch_stride != 0 && b_batch_stride != kc))
+        return fail(MPYC_B200_EINVAL, "gf_matmul_batched: a batch stride must be 0 or the matrix size");
+    if (__builtin_mul_overflow(a_batch_stride ? batch : 1, rk, &ab) || __builtin_mul_overflow(b_batch_stride ? batch : 1, kc, &bb) ||
+        ab > (size_t)INT64_MAX || bb > (size_t)INT64_MAX)
+        return fail(MPYC_B200_EINVAL, "gf_matmul_batched: size overflow");
+    if (cb == 0) return MPYC_B200_OK;
+    if (!d_c || (k && (!d_a || !d_b))) return fail(MPYC_B200_EINVAL, "gf_matmul_batched: null buffer");
+    if (bytes_overlap(d_c, cb, d_a, ab) || bytes_overlap(d_c, cb, d_b, bb))
+        return fail(MPYC_B200_EINVAL, "gf_matmul_batched: c overlaps an operand");
+    return launch_status(launch_gf_matmul_batched(f->gf_poly, (const unsigned char*)d_a, a_batch_stride, (const unsigned char*)d_b,
+                                                  b_batch_stride, (unsigned char*)d_c, batch, r, k, c, (cudaStream_t)stream),
+                         "gf_matmul_batched launch");
+}
+
 MPYC_API int mpyc_b200_ff_binop_rows(const mpyc_b200_field* f, int op, int reflected, const void* d_a, const void* d_b, void* d_out,
                                      size_t rows, size_t cols, void* stream) {
     if (int rc = prime_only(f, "ff_binop_rows: field is null")) return rc;

@@ -12,6 +12,8 @@
 
 #include <atomic>
 
+#include "gf_ops.h"
+
 extern std::atomic<unsigned long long> g_mpyc_launches;
 int mpyc_grid_size(const void* kernel, size_t items, size_t dyn_smem);
 
@@ -25,27 +27,6 @@ struct GfTab {
 struct GfRows {
     const unsigned char* p[64];
 };
-
-__host__ __device__ __forceinline__ unsigned gf_mul1(unsigned a, unsigned b, unsigned poly) {
-    unsigned acc = 0;
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        acc ^= (b & 1u) ? a : 0u;
-        b >>= 1;
-        a <<= 1;
-        if (a & 0x100u) a ^= poly;
-    }
-    return acc & 0xFFu;
-}
-
-__host__ __device__ __forceinline__ unsigned gf_pow1(unsigned a, unsigned long long e, unsigned poly) {
-    unsigned r = 1;
-    for (int i = 63; i >= 0; i--) {
-        r = gf_mul1(r, r, poly);
-        if ((e >> i) & 1ull) r = gf_mul1(r, a, poly);
-    }
-    return r;
-}
 
 // 8 bytes at a time: multiply every byte of a by x
 __device__ __forceinline__ unsigned long long gf_xtime8(unsigned long long a, unsigned long long red) {

@@ -132,6 +132,15 @@ cudaError_t launch_all_any_axis(const FieldParams& fp, const u64* in, u64* out, 
 cudaError_t launch_matmul_int(const FieldParams& fp, const u64* X, const u64* W, bool w_unsigned, bool w_left, u64* C, size_t r,
                               size_t k, size_t c, cudaStream_t st);
 
+// K15 (inst_gf.cu), GF(2^8) bytes: out[i] = sum_j x[i l + j] X^j mod poly (l >= 1); out = a_view (op) b_view, op OP_ADD / OP_SUB
+// (both XOR) or OP_MUL; C[b] (r x c) = A + b as (r x k) @ B + b bs (k x c), a batch stride 0 broadcasting its side.  Sizes
+// validated by the caller.
+cudaError_t launch_gf_bits_compose(unsigned poly, const unsigned char* x, size_t n, size_t l, unsigned char* out, cudaStream_t st);
+cudaError_t launch_gf_binop_view(unsigned poly, int op, const BinopPlan& pl, const unsigned char* a, const unsigned char* b,
+                                 unsigned char* out, cudaStream_t st);
+cudaError_t launch_gf_matmul_batched(unsigned poly, const unsigned char* A, size_t as, const unsigned char* B, size_t bs,
+                                     unsigned char* C, size_t batch, size_t r, size_t k, size_t c, cudaStream_t st);
+
 extern template struct Launch<1>;
 extern template struct Launch<2>;
 extern template struct Launch<3>;

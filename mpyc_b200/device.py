@@ -581,6 +581,47 @@ def binop_view(a: DeviceArray, a_view, b: DeviceArray, b_view, op):
     return out
 
 
+# ---- K15: GF(2^8) bit composition, broadcast arithmetic and stacked products (csrc/gf_local.cuh) ----------------------
+
+def gf_bits_compose(bits: DeviceArray, n, l):
+    """out[i] = sum_j bits[i l + j] X^j mod poly over GF(2^8), bits (n, l) row-major: np.sum(v << np.arange(l), axis=-1) of
+    BinaryPolynomial values reduced by field.array (mpyc/runtime.py:4415, 4483).  A DeviceArray of n elements."""
+    if bits.n != n * l:
+        raise ValueError('gf_bits_compose: shape does not match the buffer')
+    bits._check_contiguous()
+    out = DeviceArray.empty(bits.ctx, n, bits.t.device)
+    check(lib.mpyc_b200_gf_bits_compose(bits.ctx.handle, bits.ptr, n, l, out.ptr, _stream_ptr()))
+    return out
+
+
+def gf_binop_view(a: DeviceArray, a_view, b: DeviceArray, b_view, op):
+    """a[a_view] (op) b[b_view] over GF(2^8) into a new contiguous array (C order of the views' extents); op _cabi.OP_ADD /
+    OP_SUB (both XOR) / OP_MUL."""
+    if a.ctx is not b.ctx:
+        raise ValueError('gf_binop_view: arrays of different fields')
+    keep = []
+    av, bv = _view(a_view, keep), _view(b_view, keep)
+    out = DeviceArray.empty(a.ctx, a_view.size, a.t.device)
+    check(lib.mpyc_b200_gf_binop_view(a.ctx.handle, op, a.ptr, a.n, ctypes.byref(av), b.ptr, b.n, ctypes.byref(bv), out.ptr,
+                                      _stream_ptr()))
+    return out
+
+
+def gf_matmul_batched(A: DeviceArray, a_stacked, B: DeviceArray, b_stacked, batch, r, k, c):
+    """C[b] = A[b] @ B[b] over GF(2^8) for b < batch: A holds batch (a_stacked) or one r x k matrix, B batch (b_stacked) or
+    one k x c matrix, all row-major.  A DeviceArray of batch * r * c elements."""
+    if A.ctx is not B.ctx:
+        raise ValueError('gf_matmul_batched: arrays of different fields')
+    if A.n != (batch if a_stacked else 1) * r * k or B.n != (batch if b_stacked else 1) * k * c:
+        raise ValueError('gf_matmul_batched: shapes do not match the buffers')
+    A._check_contiguous()
+    B._check_contiguous()
+    out = DeviceArray.empty(A.ctx, batch * r * c, A.t.device)
+    check(lib.mpyc_b200_gf_matmul_batched(A.ctx.handle, A.ptr, r * k if a_stacked else 0, B.ptr, k * c if b_stacked else 0,
+                                          out.ptr, batch, r, k, c, _stream_ptr()))
+    return out
+
+
 # ---- K9: determinants, solves, inverses and powers of matrices (csrc/linalg.cuh) ------------------------------------
 
 def det(a: DeviceArray, batch, n):

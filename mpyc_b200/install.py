@@ -231,6 +231,15 @@ def _install_operators(finfields_module, min_size):
             r = resident.matmul(mine, other, reflected=not left, ufunc=True)
             if r is not MISS:
                 return r
+        # int_ndarray + field_array (np_to_bits' `c_bits + r_bits`) reaches np.add here: + does what the hook of __add__ does
+        if ufunc is np.add and method == '__call__' and not kwargs and len(inputs) == 2 and \
+                any(resident._int_matrix(x) for x in inputs) and any(isinstance(x, cls) for x in inputs) and \
+                getattr(resident._ctx_of(type(self)), 'binary', False):
+            left = isinstance(inputs[0], cls)
+            mine, other = (inputs[0], inputs[1]) if left else (inputs[1], inputs[0])
+            r = resident.binop(mine, other, op=_cabi.OP_ADD)
+            if r is not MISS:
+                return r
         return orig['__array_ufunc__'](self, ufunc, method, *inputs, **kwargs)
 
     def __array_function__(self, func, types, args, kwargs):

@@ -48,7 +48,7 @@ resident = False      # np_recombine / PRSS results stay limb-backed (set by ins
 min_size = 1024       # plain object-array operands of fewer elements are left to the reference's operators
 public_matmul = False  # @ / np.matmul with a NumPy integer ndarray run on K14 (set by install(public_matmul=True))
 calls = {'limb_ops': 0, 'materialised': 0, 'packed': 0, 'mod_values': 0, 'pow_exp': 0, 'prod': 0,
-         'matmul_int': 0}    # counters (tests, profiling)
+         'matmul_int': 0, 'gf_local': 0}    # counters (tests, profiling); gf_local: K15 calls
 
 
 # ---------------------------------------------------------------------------------------------
@@ -260,6 +260,22 @@ class CudaBackend:
         """store of x @ w (w_left: w @ x) mod p, x a store of r*k (w_left: k*c) elements, w a NumPy integer array"""
         dev, _ = self._dev()
         return dev.matmul_int(ctx, self.to_store(ctx, x), w, r, k, c, w_left)
+
+    # ---- K15, used by the GF(2^8) hooks and ModValue in np_to_bits / np_from_bits ----
+    def gf_bits_compose(self, ctx, bits, n, l):
+        """store of sum_j bits[i l + j] X^j mod poly for i < n"""
+        dev, _ = self._dev()
+        return dev.gf_bits_compose(self.to_store(ctx, bits), n, l)
+
+    def gf_binop_view(self, ctx, op, a, a_view, b, b_view):
+        """store of a[a_view] (op) b[b_view] over GF(2^8) in C order of the views' (broadcast) extents"""
+        dev, _ = self._dev()
+        return dev.gf_binop_view(self.to_store(ctx, a), a_view, self.to_store(ctx, b), b_view, op)
+
+    def gf_matmul_batched(self, ctx, a, a_stacked, b, b_stacked, batch, r, k, c):
+        """store of the batch products A[b] @ B[b]; a side that is not stacked holds one matrix for every b"""
+        dev, _ = self._dev()
+        return dev.gf_matmul_batched(self.to_store(ctx, a), a_stacked, self.to_store(ctx, b), b_stacked, batch, r, k, c)
 
     def conv2d(self, ctx, X, W, B, k, r, m, n, v, s):
         dev, _ = self._dev()
@@ -539,7 +555,7 @@ class ModValue:
     @property
     def T(self):
         """`r_bits.T` (runtime.py:3661): a 2-D value is transposed on the device (k_transpose)."""
-        if self.store is not None and len(self.shape) == 2:
+        if self.store is not None and len(self.shape) == 2 and not self.ctx.binary:
             r, c = self.shape
             calls['limb_ops'] += 1
             return self._new(backend.transpose(self.ctx, self._flush(), r, c), (c, r), self.exact)
@@ -599,6 +615,8 @@ class ModValue:
         """self (op) other, op in '+', '-', '*'; reflected: other (op) self."""
         if self.store is None:
             return _NUMPY_OPS[op](other, self._ints) if reflected else _NUMPY_OPS[op](self._ints, other)
+        if self.ctx.binary:
+            return self._gf_ring(other, op, reflected)
         p = self.ctx.modulus
         k = self._scalar(other)
         if k is not None:
@@ -627,6 +645,16 @@ class ModValue:
         code = {'+': _cabi.OP_ADD, '-': _cabi.OP_SUB, '*': _cabi.OP_MUL}[op]
         x, y = (b, a) if reflected else (a, b)
         return self._new(backend.binop(self.ctx, code, x, y))
+
+    def _gf_ring(self, other, op, reflected):
+        """GF(2^8): + and - of two values of one shape are XOR (`field_array + r_modl`, runtime.py:4418); anything else
+        settles."""
+        if op in '+-' and type(other) in (ModValue, LimbValue) and other.store is not None and other.ctx is self.ctx \
+                and other.shape == self.shape:
+            calls['limb_ops'] += 1
+            return self._new(backend.binop(self.ctx, _cabi.OP_ADD, self.store, other._flush() if type(other) is ModValue else other.store))
+        a = self._materialise()
+        return _NUMPY_OPS[op](other, a) if reflected else _NUMPY_OPS[op](a, other)
 
     def _ring_rows(self, other, op, reflected):
         """NumPy's row broadcast between a vector (C,) and a matrix (R, C) -- `s_sign - <matrix>` (runtime.py:3670)."""
@@ -678,7 +706,7 @@ class ModValue:
         return self
 
     def __pow__(self, e):
-        if self.store is not None and self._scalar(e) == 2 and not self._sq:
+        if self.store is not None and self._scalar(e) == 2 and not self._sq and not self.ctx.binary:
             self._flush()
             return self._new(self.store, None, False, sq=True)
         return self._materialise() ** e
@@ -687,14 +715,14 @@ class ModValue:
         if self.store is None:
             return self._ints << k
         n = self._scalar(k)
-        if n is not None and n >= 0:
+        if n is not None and n >= 0 and not self.ctx.binary:
             return self._ring(pow(2, n, self.ctx.modulus), '*')
         if (isinstance(k, np.ndarray) and type(k) is np.ndarray and k.ndim == 1 and k.dtype.kind in 'iu' and len(self.shape) >= 2
                 and k.shape[0] == self.shape[-1] and k.shape[0] > 0 and self.size):
             f = k.shape[0]
             if np.array_equal(k, np.arange(f)):
                 return _ShiftedBits(self, k, False)
-            if np.array_equal(k, np.arange(f - 1, -1, -1)):
+            if np.array_equal(k, np.arange(f - 1, -1, -1)) and not self.ctx.binary:
                 return _ShiftedBits(self, k, True)
         return self._materialise() << k
 
@@ -710,8 +738,8 @@ class ModValue:
             raise AssertionError(f'mpyc_b200: {what} on a modular intermediate (only opened / stored residues are exact)')
 
     def __and__(self, mask):
-        if self.store is None:
-            return self._ints & mask
+        if self.store is None or self.ctx.binary:
+            return self._materialise() & mask
         m = self._scalar(mask)
         if m is not None and m >= 0 and (m + 1) & m == 0:           # 2^b - 1
             self._need_exact('bit mask')
@@ -723,8 +751,8 @@ class ModValue:
     __rand__ = __and__
 
     def __mod__(self, q):
-        if self.store is None:
-            return self._ints % q
+        if self.store is None or self.ctx.binary:
+            return self._materialise() % q
         m = self._scalar(q)
         if m == self.ctx.modulus:
             return self if not self._sq and self._s == 1 and self._t == 0 else self._new(self._flush())
@@ -736,6 +764,8 @@ class ModValue:
     __imod__ = __mod__
 
     def __ne__(self, other):
+        if self.store is not None and self.ctx.binary:
+            return self._materialise() != other
         if self.store is not None and self._scalar(other) == 0:
             self._need_exact('!= 0')
             mask, _ = backend.nonzero(self.ctx, self.store)
@@ -745,6 +775,8 @@ class ModValue:
         return self._materialise() != other
 
     def __eq__(self, other):
+        if self.store is not None and self.ctx.binary:
+            return self._materialise() == other
         if self.store is not None and self._scalar(other) == 0:
             self._need_exact('== 0')                               # `c.value == 0` (runtime.py:3614)
             mask, _ = backend.nonzero(self.ctx, self.store)
@@ -762,7 +794,7 @@ class ModValue:
             if ufunc is not np.left_shift:
                 return self._ring(a, _UFUNC_OPS[ufunc], reflected=True)
         if (method == 'outer' and ufunc is np.right_shift and len(inputs) == 2 and not kwargs and inputs[0] is self
-                and self.store is not None and len(self.shape) == 1 and self.exact):
+                and self.store is not None and len(self.shape) == 1 and self.exact and not self.ctx.binary):
             k = inputs[1]
             if isinstance(k, np.ndarray) and type(k) is np.ndarray and k.ndim == 1 and k.dtype.kind in 'iu' and k.shape[0] > 0:
                 l = k.shape[0]
@@ -772,7 +804,7 @@ class ModValue:
                     return _OuterBits(self, k, True, False)
         if method in ('__call__', 'outer') and ufunc in (np.right_shift, np.bitwise_and, np.not_equal, np.equal, np.remainder):
             for x in inputs:
-                if type(x) is ModValue and x.store is not None:
+                if type(x) is ModValue and x.store is not None and not x.ctx.binary:
                     x._need_exact(ufunc.__name__)
         args = [x._materialise() if type(x) in (ModValue, LimbValue) else x for x in inputs]
         if 'out' in kwargs:
@@ -782,6 +814,8 @@ class ModValue:
     def __array_function__(self, func, types, args, kwargs):
         """np.vstack / np.cumsum(axis=0) of 2-D values stay on the device (runtime.py:3667-3670); every other NumPy
         function gets the settled object arrays."""
+        if self.ctx.binary:
+            return func(*_settled(args), **_settled(kwargs))
         if func is np.vstack and len(args) == 1 and not kwargs:
             r = _vstack(self.ctx, args[0])
             if r is not None:
@@ -955,6 +989,9 @@ class _ShiftedBits:
             f = b.shape[-1]                              # the bit positions are the last axis (runtime.py:860, 4415)
             n = b.size // f
             calls['limb_ops'] += 1
+            if b.ctx.binary:
+                calls['gf_local'] += 1
+                return b._new(backend.gf_bits_compose(b.ctx, b._flush(), n, f), b.shape[:-1])
             return b._new(backend.bits_compose(b.ctx, b._flush(), n, f, self.descending), b.shape[:-1])
         return self._eval().sum(axis=axis, out=out, **kwargs)
 
@@ -1046,6 +1083,7 @@ def as_limb_value(value):
 _slot = None            # the member descriptor FiniteFieldArray.__dict__['value'] of the patched finfields module
 _lazy_codes = set()     # code objects that may see a LimbValue (see module docstring)
 _mod_codes = set()      # code objects that get a ModValue: their arithmetic on raw values runs mod p on the device
+_gf_mod_codes = set()   # those of _mod_codes that get a ModValue over GF(2^8) as well (_GF_MOD_NAMES)
 _runtime_seen = [False]
 local_algebra = True    # hand ModValues to the functions below (install(local_algebra=...))
 
@@ -1062,6 +1100,9 @@ _MOD_SOURCES = {
     '_np_is_zero': 'd2beb72e8b098a8e79dbdd2438f24e0972b9a6c46073fbad7a13bec0a6c761f0',        # runtime.py:3581-3620
     'np_from_bits': '64d71aeb3dbed028a8046d6176b2fd8c8b38661bcd831ee069d3d1749338956c',       # runtime.py:4475-4484
 }
+# Over GF(2^8) (with K15) only these get ModValues: their raw-value algebra there is `v << np.arange(l)` summed along the last
+# axis (k_gf_bits_compose), `field_array + r_modl` (XOR) and reads of the opened `c` (runtime.py:4415-4423, 4483).
+_GF_MOD_NAMES = ('np_to_bits', 'np_from_bits')
 
 
 def raw_value(arr):
@@ -1097,6 +1138,8 @@ def _collect_runtime_codes(finfields_module):
             try:
                 if hashlib.sha256(inspect.getsource(fn).encode()).hexdigest() == digest:
                     _mod_codes.add(fn.__code__)
+                    if name in _GF_MOD_NAMES:
+                        _gf_mod_codes.add(fn.__code__)
             except (OSError, TypeError):
                 pass
     _runtime_seen[0] = True
@@ -1109,6 +1152,7 @@ def make_value_property(finfields_module):
     slot_get, slot_set = _slot.__get__, _slot.__set__
     _lazy_codes.clear()
     _mod_codes.clear()
+    _gf_mod_codes.clear()
     _runtime_seen[0] = False
     for name in ('reshape', 'ravel', 'flatten', 'copy', '__len__'):
         fn = cls.__dict__.get(name)
@@ -1130,7 +1174,7 @@ def make_value_property(finfields_module):
             code = sys._getframe(1).f_code
             if code in _lazy_codes:
                 return v
-            if code in _mod_codes and not v.ctx.binary:
+            if code in _mod_codes and (not v.ctx.binary or (code in _gf_mod_codes and _gf_backend())):
                 calls['mod_values'] += 1
                 return ModValue(v.ctx, v.store, v.shape, exact=True)
         a = v._materialise()
@@ -1163,7 +1207,8 @@ def _ctx_of(cls):
 
 def _operand(ctx, cls, x, any_size=False):
     """(store, shape) of an array operand as limbs, or None when it should stay with the reference's code.  An object array
-    of Python ints is packed when it has at least min_size elements, or whatever its size with any_size."""
+    of Python ints is packed when it has at least min_size elements, or whatever its size with any_size; over GF(2^8) (with
+    K15) an object array of BinaryPolynomial or non-negative int entries, each reduced by _gf2_mod."""
     if isinstance(x, cls):
         x = raw_value(x)
     lv = as_limb_value(x)
@@ -1171,10 +1216,34 @@ def _operand(ctx, cls, x, any_size=False):
         return (lv.store, lv.shape) if lv.ctx is ctx else None
     if type(x) is LimbValue or type(x) is ModValue:
         x = x._ints
-    if isinstance(x, np.ndarray) and x.dtype == object and (any_size or x.size >= min_size) and not ctx.binary:
-        calls['packed'] += 1
-        return codec.ints_to_limbs(x.reshape(-1), ctx), x.shape
+    if isinstance(x, np.ndarray) and x.dtype == object and (any_size or x.size >= min_size):
+        if not ctx.binary:
+            calls['packed'] += 1
+            return codec.ints_to_limbs(x.reshape(-1), ctx), x.shape
+        store = _gf_bytes(ctx, x, type(cls.field.modulus)) if _gf_backend() else None
+        if store is not None:
+            calls['packed'] += 1
+            return store, x.shape
     return None
+
+
+def _gf_backend():
+    """K15's hooks run only when the backend has its three methods.  CudaBackend always does; a substituted backend without
+    them (a test stand-in) leaves GF(2^8) operands to the reference's code, as before K15 existed."""
+    return all(hasattr(backend, m) for m in ('gf_bits_compose', 'gf_binop_view', 'gf_matmul_batched'))
+
+
+def _gf_bytes(ctx, x, poly_type):
+    """uint8 store of an object array of polynomial (poly_type: the field's BinaryPolynomial class) or non-negative int
+    entries reduced mod the field polynomial (the reference's field.array reduces them so, finfields.py:724); None when
+    another entry occurs."""
+    out = np.empty(x.size, dtype=np.uint8)
+    for i, v in enumerate(x.flat):
+        if not (isinstance(v, poly_type) or
+                (isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_)) and v >= 0)):
+            return None
+        out[i] = _gf2_mod(int(v), ctx.modulus)
+    return out
 
 
 def _qualifies(value):
@@ -1229,14 +1298,14 @@ def binop(self, other, op, reflected=False):
         return _wrap(cls, ctx, backend.binop_scalar(ctx, op, a[0], s), a[1])
     if not isinstance(other, (cls, np.ndarray, LimbValue)):
         return _MISS
-    b = _operand(ctx, cls, other)
+    b = _gf_int_operand(ctx, self, other, op) if _int_matrix(other) else _operand(ctx, cls, other)
     if b is None:
         return _MISS
     if b[1] != a[1]:
         # NumPy's row broadcast between a matrix (R, C) and a vector (C,) runs on k_binop_rows, any other broadcast on
-        # K8's k_binop_view
+        # K8's k_binop_view (K15's k_gf_binop_view over GF(2^8))
         if ctx.binary:
-            return _MISS
+            return _broadcast_binop(cls, ctx, op, (b, a) if reflected else (a, b))
         if len(a[1]) == 2 and len(b[1]) == 1 and a[1][1] == b[1][0] and a[1][0] and a[1][1]:
             mat, vec, vec_first = a, b, reflected
         elif len(a[1]) == 1 and len(b[1]) == 2 and b[1][1] == a[1][0] and b[1][0] and b[1][1]:
@@ -1259,7 +1328,7 @@ def _broadcast_binop(cls, ctx, op, operands):
     """x (op) y under NumPy broadcasting for stores x, y of two shapes (K8's k_binop_view; the broadcast operand is read in
     place); _MISS for incompatible shapes (NumPy raises) and views beyond the kernels' rank."""
     (x, sx), (y, sy) = operands
-    if not _layout_backend():
+    if not (_gf_backend() if ctx.binary else _layout_backend()):
         return _MISS
     try:
         shape, vx, vy = layout.broadcast_views(sx, sy)
@@ -1268,7 +1337,21 @@ def _broadcast_binop(cls, ctx, op, operands):
     c = layout.collapse(vx, vy)
     if c is None:
         return _MISS
-    return _wrap(cls, ctx, backend.binop_view(ctx, op, x, c[0], y, c[1]), shape)
+    view_op = backend.gf_binop_view if ctx.binary else backend.binop_view
+    calls['gf_local'] += ctx.binary
+    return _wrap(cls, ctx, view_op(ctx, op, x, c[0], y, c[1]), shape)
+
+
+def _gf_int_operand(ctx, self, other, op):
+    """(store, shape) of a NumPy integer ndarray added to a limb-backed GF(2^8) array -- np_to_bits' `c_bits + r_bits`
+    (runtime.py:4423): entries in [0, 256) are the field elements with those encodings, uploaded as bytes.  None for other
+    entries, other operations, prime fields and backends without K15."""
+    if not ctx.binary or op != _cabi.OP_ADD or not _gf_backend() or as_limb_value(raw_value(self)) is None or not other.size:
+        return None
+    if other.min() < 0 or other.max() > 255:
+        return None
+    calls['packed'] += 1
+    return np.ascontiguousarray(other, dtype=np.uint8).reshape(-1), other.shape
 
 
 def _element(cls, ctx, store):
@@ -1401,8 +1484,8 @@ def swapaxes(self, axis1, axis2):
 
 
 def _join_parts(cls, arrays):
-    """[(shape, LimbValue or None)] of a join's pieces -- arrays of class cls, limb-backed or (prime fields) of Python ints
-    (None), at least one limb-backed -- or None."""
+    """[(shape, LimbValue or None)] of a join's pieces -- arrays of class cls, limb-backed or plain (None: Python ints, or
+    over GF(2^8) with K15 polynomials, packed by _operand), at least one limb-backed -- or None."""
     if not isinstance(arrays, (list, tuple)) or not arrays or any(type(a) is not cls for a in arrays):
         return None
     ctx = _ctx_of(cls)
@@ -1414,7 +1497,7 @@ def _join_parts(cls, arrays):
     for v, x in zip(lvs, vals):
         if v is not None:
             parts.append((v.shape, v))
-        elif isinstance(x, np.ndarray) and x.dtype == object and not ctx.binary:
+        elif isinstance(x, np.ndarray) and x.dtype == object and (not ctx.binary or _gf_backend()):
             parts.append((x.shape, None))
         else:
             return None
@@ -1578,8 +1661,10 @@ def matmul(self, other, reflected=False, ufunc=False):
         v = raw_value(x) if isinstance(x, cls) else x
         return getattr(v, 'shape', None)
     sa, sb = shape_of(A), shape_of(B)
-    if sa is None or sb is None or not (1 <= len(sa) <= 2 and 1 <= len(sb) <= 2):
+    if sa is None or sb is None or not sa or not sb:
         return _MISS
+    if len(sa) > 2 or len(sb) > 2:
+        return _gf_matmul_stacked(cls, ctx, A, B, sa, sb) if ctx.binary and not _int_matrix(other) else _MISS
     r, k = (1, sa[0]) if len(sa) == 1 else sa
     k2, c = (sb[0], 1) if len(sb) == 1 else sb
     if k != k2:
@@ -1607,6 +1692,41 @@ def matmul(self, other, reflected=False, ufunc=False):
         v = LimbValue(ctx, out, (1,), poly)._materialise()[0]
         return cls(np.array(v, dtype=object), check=False) if ufunc else cls.field(v)
     shape = (c,) if len(sa) == 1 else ((r,) if len(sb) == 1 else (r, c))
+    return _wrap(cls, ctx, out, shape)
+
+
+def _gf_matmul_stacked(cls, ctx, A, B, sa, sb):
+    """A @ B over GF(2^8) with an operand of more than two axes (NumPy's matmul of stacks, the S-box's `A @ x[..., None]`) on
+    K15's k_gf_matmul_batched: each side's stack axes either match the broadcast stack shape or hold one matrix (stride 0).
+    _MISS for partial broadcasts of the stack axes, empty results, mismatched shapes (NumPy raises), backends without K15 and
+    plain operands below the size rule."""
+    if not _gf_backend():
+        return _MISS
+    a2 = sa if len(sa) >= 2 else (1,) + sa
+    b2 = sb if len(sb) >= 2 else sb + (1,)
+    (r, k), (k2, c) = a2[-2:], b2[-2:]
+    try:
+        stack = np.broadcast_shapes(a2[:-2], b2[:-2])
+    except ValueError:
+        return _MISS
+    batch = layout._prod(stack)
+    if k != k2 or not batch * r * c:
+        return _MISS
+    stacked = []
+    for s in (a2[:-2], b2[:-2]):
+        full = (1,) * (len(stack) - len(s)) + tuple(s) == tuple(stack)
+        if not full and layout._prod(s) != 1:
+            return _MISS
+        stacked.append(full and batch > 1)
+    limbish = any(isinstance(x, cls) and as_limb_value(raw_value(x)) is not None for x in (A, B))
+    if not limbish and batch * r * k * c < min_size * 8:
+        return _MISS
+    a, b = _operand(ctx, cls, A, any_size=True), _operand(ctx, cls, B, any_size=True)
+    if a is None or b is None:
+        return _MISS
+    calls['gf_local'] += 1
+    out = backend.gf_matmul_batched(ctx, a[0], stacked[0], b[0], stacked[1], batch, r, k, c)
+    shape = tuple(stack) + ((r,) if len(sa) >= 2 else ()) + ((c,) if len(sb) >= 2 else ())
     return _wrap(cls, ctx, out, shape)
 
 
